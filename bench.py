@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- Hψ applies/s (and SCF-step pieces) of the B200 plane-wave Kohn-Sham hot path.
+"""bench.py -- Hψ applies/s (and SCF-step pieces) of the plane-wave Kohn-Sham hot path on an H100 (sm_90a).
 
 Contract: `python bench.py --gpus N --steps K --warmup W [--impl reference]` prints ONE JSON line
 (rank 0).  A *step* is one full Hamiltonian application `mul!(Hψ, H::DftHamiltonianBlock, ψ)` on the block
 of M bands of one k-block (batched FFT local part + kinetic + nonlocal P D P†ψ).
 
-Workload at N=1: BASELINE.json configs[2] -- Si 5x5x5 supercell (250 atoms, 1000 e-), LDA, Γ only,
-Ecut = 30 Ha, fft 192³, N_pw = 264 859, M = 503 bands, n_proj = 1250 (the configuration the north-star
-targets are quoted on).  For N>1 every rank owns one k-block of that shape (k-points shard; weak scaling):
-no data-path collective inside Hψ; the density allreduce of an SCF step is timed separately.
+Workload at N=1: Si 4x4x4 supercell (128 atoms, 512 e-), LDA, Γ only, Ecut = 30 Ha, M = 259 bands,
+n_proj = 640: the largest silicon supercell of this family whose LOBPCG and SCF sections fit the 80 GB of one H100
+(the 5x5x5 cell of BASELINE.json configs[2], 503 bands at N_pw = 264 859, does not).  For N>1 every rank owns one
+k-block of that shape (k-points shard; weak scaling): no data-path collective inside Hψ; the density allreduce of an SCF
+step is timed separately.
 
 `value`  = band-applies/s with ψ/Hψ resident in HBM (CUDA events, max over ranks).
 `e2e`    = the same call through the C ABI with pinned HOST ψ/Hψ buffers (H2D + D2H inside the timed region).
@@ -17,6 +18,10 @@ no data-path collective inside Hψ; the density allreduce of an SCF step is time
 `roofline_gemm` = the nonlocal P D P†ψ GEMMs (FP64 DMMA; 16·N_pw·n_proj·M flop) against a cuBLAS ZGEMM
              probe measured in the same run (MEASURED_PEAKS.json has no FP64 figure).
 `cpu_baseline` = the CPU oracle (port of the reference's band-at-a-time algorithm) on a bounded sample.
+
+`--dump-outputs DIR` writes what the timed H apply returned in its last step: a fixed, seeded sample of Hψ
+(`hpsi_sample.npy`, float64 [re, im] pairs, at the flat indices of `hpsi_sample_index.npy`) and the norm of every band
+of Hψ (`hpsi_band_norms.npy`).  The inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -59,7 +64,7 @@ import numpy as np
 A_SI = 10.26 / 2
 WORKLOADS = {
     # name: (supercell repeat, Ecut, n_bands)
-    "si250": dict(rep=5, Ecut=30.0, desc="Si 5x5x5 supercell (250 atoms) LDA Gamma Ecut=30 Ha, fft 192^3"),
+    "si128": dict(rep=4, Ecut=30.0, desc="Si 4x4x4 supercell (128 atoms) LDA Gamma Ecut=30 Ha"),
     "si16": dict(rep=2, Ecut=30.0, desc="Si 2x2x2 supercell (16 atoms) LDA Gamma Ecut=30 Ha (dev/smoke size)"),
     "si2": dict(rep=1, Ecut=30.0, desc="Si 2-atom primitive LDA Ecut=30 Ha (dev/smoke size)"),
 }
@@ -85,8 +90,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "MEASURED_PEAKS.json hbm_gbs (driver-measured copy bandwidth)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "MEASURED_PEAKS.json hbm_gbs (of measured copy bandwidth)"
+    return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3"
 
 
 class ClockSampler:
@@ -317,6 +322,17 @@ def library_gpu_baseline(torch, basis, blk, kb, psi, n_local_bands):
 
 
 # ---------------------------------------------------------------------------------------------- GPU arm
+def dump_outputs(out_dir, torch, hpsi, n_sample=1 << 20):
+    """Hψ of the last timed step: a seeded sample of 2^20 entries (flat band-major indices) and every band's norm."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = hpsi.numel()
+    idx = np.unique(np.random.default_rng(2024).integers(0, total, size=min(n_sample, total)))
+    vals = torch.view_as_real(hpsi.reshape(-1)[torch.from_numpy(idx).to(hpsi.device)]).cpu().numpy()
+    np.save(os.path.join(out_dir, "hpsi_sample.npy"), vals.astype(np.float64))
+    np.save(os.path.join(out_dir, "hpsi_sample_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "hpsi_band_norms.npy"), torch.linalg.vector_norm(hpsi, dim=1).cpu().numpy().astype(np.float64))
+
+
 def run_gpu(args):
     # Keep stdout clean for the single JSON line: C libraries (e.g. the NCCL version banner) write to fd 1.
     saved_stdout = os.dup(1)
@@ -388,6 +404,8 @@ def run_gpu(args):
     clocks = sampler.stop() if sampler else None
     ms_step = ms_total / args.steps
     value = world * M * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, hpsi)
 
     # ---- kernel-group breakdown (same stream, CUDA events)
     ms_local = timed(lambda: kb.apply_terms(psi, 3, out=hpsi), max(2, args.steps // 2), 1) / max(2, args.steps // 2)
@@ -395,37 +413,27 @@ def run_gpu(args):
     hbm_peak, peak_src = peaks()
     alg_bytes_band = 72.0 * N + 40.0 * n_pw
     ach = alg_bytes_band * M / (ms_local * 1e-3) / 1e9
-    # measured DRAM traffic of the group (dram__bytes_read.sum + dram__bytes_write.sum over the five kernels of one
-    # `ncu --set full` capture, profiles/ncu_full_r1.csv: 17.11 GB per 51-band launch on the 192^3 grid), scaled to the
-    # block like `achieved`; only known for the profiled workload
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")       # written by scripts/summarize_ncu.py from the round's
-    if args.workload == "si250" and os.path.exists(tpath):            # `ncu --set full` capture (dram bytes read + written)
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj["hpsi_local_dram_bytes_per_band"] * M, tj["source"]
     roofline = dict(bound="hbm", kernel="Hpsi-local group (kr_sphere_to_x, kr_y_backward, kr_z_apply, kr_y_forward, kr_x_to_sphere)",
-                    achieved=ach, peak=hbm_peak, unit="GB/s", frac=ach / hbm_peak, traffic=traffic,
-                    traffic_source=traffic_src,
+                    achieved=ach, peak=hbm_peak, unit="GB/s", frac=ach / hbm_peak,
                     algorithmic_bytes_per_band=alg_bytes_band, ms_per_block=ms_local, us_per_band=1e3 * ms_local / M,
-                    peak_source=peak_src + " (of measured)")
+                    peak_source=peak_src)
     n_proj = kb.n_proj
     fl_nl = 16.0 * n_pw * n_proj * M
-    # the same two projector products on the FP64 DMMA pipe: own kernels (gemm_backend 0) and cuBLAS ZGEMM (gemm_backend 1, the
-    # FP64 peak calibration; MEASURED_PEAKS.json has no FP64 figure).  The default path (gemm_backend 4) runs them on the INT8
-    # tensor cores (tcgen05.mma.kind::i8, exact FP64-equivalent results through residues + CRT), so `frac` can exceed 1.
-    backend_default = 4
+    # the default path runs the two projector products on the own FP64 DMMA kernels (gemm_backend 0); beside it cuBLAS ZGEMM
+    # (gemm_backend 1, the FP64 peak calibration; MEASURED_PEAKS.json has no FP64 figure) and the INT8 tensor-core path
+    # (gemm_backend 4: wgmma s8, exact FP64-equivalent results through residues + CRT) on the same shapes
+    backend_default = 0
     ctx.set_option("gemm_backend", 1)
     ms_nl_cublas = timed(lambda: kb.apply_terms(psi, 4, out=hpsi), 2, 1) / 2
-    ctx.set_option("gemm_backend", 0)
-    ms_nl_dmma = timed(lambda: kb.apply_terms(psi, 4, out=hpsi), 2, 1) / 2
+    ctx.set_option("gemm_backend", 4)
+    ms_nl_i8 = timed(lambda: kb.apply_terms(psi, 4, out=hpsi), 2, 1) / 2
     ctx.set_option("gemm_backend", backend_default)
-    tf_nl, tf_cublas, tf_dmma = (fl_nl / (t * 1e-3) / 1e12 for t in (ms_nl, ms_nl_cublas, ms_nl_dmma))
-    roofline_gemm = dict(bound="tensor", kernel="nonlocal P D P'psi: k_i8_gemm_tc2 + k_i8_gemm_tc2_nn (tcgen05.mma.kind::i8, TMA-fed, INT8 residues + CRT) "
-                                                "with k_i8_residues_ld4 / k_i8_crt_nn around them",
-                         achieved=tf_nl, peak=tf_cublas, unit="TFLOP/s (FP64-equivalent)", frac=tf_nl / tf_cublas, flop=fl_nl, ms=ms_nl,
-                         peak_source="cuBLAS ZGEMM (FP64 DMMA pipe) on the same shapes in the same run; nominal FP64 tensor 37-40 TFLOP/s",
-                         own_dmma_kernels=dict(ms=ms_nl_dmma, achieved=tf_dmma, frac_of_cublas=tf_dmma / tf_cublas, frac_of_fixed_36TF=tf_dmma / 36.0),
-                         tensor_pipe_evidence="profiles/ncu_i8_r2.csv: sm__pipe_tensor_cycles_active of k_i8_gemm_tc2 / k_i8_gemm_tc2_nn")
+    tf_nl, tf_cublas, tf_i8 = (fl_nl / (t * 1e-3) / 1e12 for t in (ms_nl, ms_nl_cublas, ms_nl_i8))
+    roofline_gemm = dict(bound="tensor", kernel="nonlocal P D P'psi: own FP64 DMMA kernels (k_zgemm_cn, k_zgemm_nn)",
+                         achieved=tf_nl, peak=tf_cublas, unit="TFLOP/s", frac=tf_nl / tf_cublas, flop=fl_nl, ms=ms_nl,
+                         peak_source="cuBLAS ZGEMM (FP64 DMMA pipe) on the same shapes in the same run",
+                         int8_tensor_cores=dict(ms=ms_nl_i8, achieved=tf_i8, unit="TFLOP/s (FP64-equivalent)", frac_of_cublas=tf_i8 / tf_cublas,
+                                                kernel="k_i8_gemm_tc2 + k_i8_gemm_tc2_nn (wgmma s8, TMA-fed) with k_i8_residues_ld4 / k_i8_crt_nn"))
     # ---- the reference's GPU formulation with library kernels (cuFFT band-at-a-time + cuBLAS) on the same block
     lib_gpu = None
     if rank == 0 and not args.no_library:
@@ -498,12 +506,14 @@ def run_gpu(args):
         except Exception as e:
             extra["lobpcg"]["gemm_flop_error"] = repr(e)
         del X
+        kb.trim()       # the solve's scratch: the SCF below solves its own copy of this block, and both do not fit in 80 GB
+        torch.cuda.empty_cache()
 
     # ---- single-k multi-GPU (SURVEY §8 f3): the SAME Gamma block solved by all ranks together (plane-wave slabs: local Gram
     #      products + NCCL allreduce, rows <-> bands exchange around H) against one GPU solving it alone, same start vectors
     if world > 1 and args.scf and not args.no_slab:
         try:
-            kb.trim()        # the 503-band solve above left ~60 GB of solver scratch on this rank's k-block
+            kb.trim()        # the solve above left its solver scratch on this rank's k-block
             torch.cuda.empty_cache()
             bs = dftk.PlaneWaveBasis(model, Ecut=w["Ecut"], kgrid=(1, 1, 1), architecture=arch, comm_slab=comm)
             hs = dftk.energy_hamiltonian(bs, None, None, rho=dftk.guess_density(bs))[1]
@@ -719,7 +729,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--workload", default=os.environ.get("DFTK_BENCH_WORKLOAD", "si250"), choices=list(WORKLOADS))
+    ap.add_argument("--workload", default=os.environ.get("DFTK_BENCH_WORKLOAD", "si128"), choices=list(WORKLOADS))
     ap.add_argument("--bands", type=int, default=0)
     ap.add_argument("--cpu-bands", type=int, default=0,
                     help="bands in the CPU sample (0 = 64)")
@@ -737,6 +747,8 @@ def main():
     ap.add_argument("--slab-scf-steps", type=int, default=0, help="SCF iterations of the single-k slab section when --scf-steps is 0")
     ap.add_argument("--scf-tol", type=float, default=0.025)
     ap.add_argument("--scf-maxiter", type=int, default=6)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the H psi of the last timed step (seeded sample + band norms) as .npy files to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else max(args.warmup, 1)
     if args.cpu_bands <= 0:

@@ -1,4 +1,4 @@
-"""dftk_b200: B200-native plane-wave Kohn-Sham SCF hot path behind DFTK.jl's operator API.
+"""dftk_b200: H100-native (sm_90a) plane-wave Kohn-Sham SCF hot path behind DFTK.jl's operator API.
 
 The package directory is `dftk.jl_b200/`; import it as `dftk_b200` (see dftk_b200.py at the repo root).
 Names follow the reference (Model, PlaneWaveBasis, self_consistent_field, HamiltonianBlock, ...).

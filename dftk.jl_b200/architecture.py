@@ -14,7 +14,7 @@ class AbstractArchitecture:
 
 class CPU(AbstractArchitecture):
     def __init__(self):
-        raise NotImplementedError("dftk_b200 is the B200 back end only; use DFTK.jl itself for CPU runs")
+        raise NotImplementedError("dftk_b200 is a GPU back end only; use DFTK.jl itself for CPU runs")
 
 
 class B200(AbstractArchitecture):

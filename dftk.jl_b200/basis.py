@@ -1,6 +1,6 @@
 """PlaneWaveBasis / Kpoint / MonkhorstPack (host-side mirror of src/PlaneWaveBasis.jl:129-369,
 src/Kpoint.jl:6-74, src/bzmesh.jl:41-95, src/fft.jl:231-337).  Setup code; heavy arrays are torch
-tensors on the B200, every transform goes through libdftk_b200's own FFT kernels."""
+tensors on the GPU, every transform goes through libdftk_b200's own FFT kernels."""
 import math
 from fractions import Fraction
 import numpy as np

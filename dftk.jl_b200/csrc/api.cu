@@ -107,7 +107,7 @@ static int ctx_create_common(int device, dftk_b200_ctx** out) {
   CUDA_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-  REQUIRE(prop.major >= 10, "libdftk_b200 is built for sm_100a (Blackwell) only");
+  REQUIRE(prop.major == 9 && prop.minor == 0, "libdftk_b200 is built for sm_90a (Hopper) only");
   dftk_b200_ctx* c = new dftk_b200_ctx();
   c->device = device;
   c->sm_count = prop.multiProcessorCount;
@@ -119,7 +119,6 @@ static int ctx_create_common(int device, dftk_b200_ctx** out) {
   fft_set_attributes();
   reg_set_attributes();
   blas_set_attributes();
-  i8tc_set_attributes();
   i8tc2_set_attributes();
   lobpcg_set_attributes();
   *out = c;
@@ -235,7 +234,10 @@ int dftk_b200_set_option(dftk_b200_ctx* ctx, const char* name, int64_t value) {
   API_BEGIN
   REQUIRE(ctx && name, "set_option: NULL argument");
   std::string n(name);
-  if (n == "gemm_backend") ctx->gemm_backend = (int)value;
+  if (n == "gemm_backend") {
+    REQUIRE(value == 0 || value == 1 || value == 2 || value == 4, "set_option: gemm_backend must be 0, 1, 2 or 4");
+    ctx->gemm_backend = (int)value;
+  }
   else if (n == "band_chunk") ctx->band_chunk = (int)value;
   else if (n == "gemm_stages") ctx->gemm_stages = (value == 3 ? 3 : 2);
   else if (n == "small_dense") ctx->small_dense = (int)value;

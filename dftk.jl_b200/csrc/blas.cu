@@ -387,9 +387,9 @@ void zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_t k, cplx
     ctx->launches++;
     return;
   }
-  if ((ctx->gemm_backend == 2 || ctx->gemm_backend == 3 || (ctx->gemm_backend == 4 && k >= ctx->i8_min_rows && m >= 32 && n >= 32)) && transA == 2 && k > 0 && alpha.x == 1.0 && alpha.y == 0.0 && beta.x == 0.0 && beta.y == 0.0) {
-    // experimental: FP64 by INT8 residues + CRT (i8emu.cu; reference pipeline, groundwork for a tcgen05 kind::i8 kernel)
-    zgemm_i8_cn(ctx, m, n, k, A, lda, B, ldb, C, ldc, ctx->gemm_backend - 2);
+  if ((ctx->gemm_backend == 2 || (ctx->gemm_backend == 4 && k >= ctx->i8_min_rows && m >= 32 && n >= 32)) && transA == 2 && k > 0 && alpha.x == 1.0 && alpha.y == 0.0 && beta.x == 0.0 && beta.y == 0.0) {
+    // FP64 by INT8 residues + CRT (i8emu.cu): integer products on the tensor cores (4) or the CUDA-core reference pipeline (2)
+    zgemm_i8_cn(ctx, m, n, k, A, lda, B, ldb, C, ldc, ctx->gemm_backend == 4);
     return;
   }
   if (ctx->gemm_backend == 4 && transA == 0 && m >= ctx->i8_min_rows && k >= 32 && n >= 16 && alpha.y == 0.0 && beta.y == 0.0 && !upper_only) {
@@ -459,7 +459,7 @@ void kb_apply_nonlocal(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_
   cplx* dproj = proj + (size_t)np * n_bands;
   const cplx one = make_double2(1.0, 0.0), zero = make_double2(0.0, 0.0);
   if (ctx->gemm_backend == 4 && np >= 64 && n_bands >= 32 && kb->n_pw >= ctx->i8_min_rows) {
-    // both projector products on the INT8 tensor cores (tcgen05.mma.kind::i8, TMA-fed; i8emu.cu / i8tc2.cu): the residue
+    // both projector products on the INT8 tensor cores (wgmma s8, TMA-fed; i8emu.cu / i8tc2.cu): the residue
     // planes of P are prepared once per k-block and serve P'psi (K-major operand) and P (D P'psi) (MN-major operand)
     if (!kb->i8_Pop.planes) kb->i8_Pop = i8_prepare(ctx, kb->P.p, kb->n_pw, np, kb->n_pw, kb->i8_planes, kb->i8_exps);
     const I8Operand op_psi = i8_prepare(ctx, psi, kb->n_pw, n_bands, kb->n_pw, kb->i8_psi_planes, kb->i8_psi_exps);

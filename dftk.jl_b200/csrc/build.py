@@ -1,11 +1,11 @@
-"""Build libdftk_b200.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+"""Build libdftk_b200.so in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["fft.cu", "blas.cu", "lobpcg.cu", "api.cu", "xc.cu", "forces.cu", "setup.cu", "i8emu.cu", "i8tc.cu", "i8tc2.cu"]
+SOURCES = ["fft.cu", "blas.cu", "lobpcg.cu", "api.cu", "xc.cu", "forces.cu", "setup.cu", "i8emu.cu", "i8tc2.cu"]
 REG_NGROUPS = 4
 HEADERS = ["common.cuh", "structs.cuh", "fft_core.cuh", "fft_plan.h", "fft_reg.cuh", "fft_reg_fwd.cuh", "fft_reg.cu",
            "fft_radix_gen.cuh", "xc_core.cuh", "forces_core.cuh", "lobpcg_small.cuh", "lobpcg_batch.cuh", "i8emu_core.cuh", os.path.join("..", "..", "include", "dftk_b200.h")]
@@ -28,7 +28,7 @@ def build(force=False, verbose=False):
     lib = os.path.abspath(LIB)
     if not force and os.path.exists(lib) and os.path.getmtime(lib) >= newest:
         return lib
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
              "-Xcompiler", "-fPIC", "-I", inc, "-Wno-deprecated-gpu-targets"]
     if verbose:
         flags += ["-Xptxas", "-v"]

@@ -90,18 +90,20 @@ struct dftk_b200_ctx {
   ncclComm_t nccl = nullptr;
   int rank = 0, nranks = 1;
   int64_t launches = 0;
-  int gemm_backend = 4;   // 4 (default) = INT8 tensor cores (tcgen05.mma.kind::i8, TMA-fed; i8emu.cu / i8tc2.cu) for contractions of at least
-                          // i8_min_rows rows, own FP64 DMMA kernels otherwise; 0 = DMMA kernels only; 1 = cuBLAS (A/B comparison only);
-                          // 2 / 3 = checkers of the INT8 scheme (CUDA-core pipeline / cp.async-fed tensor-core kernel)
+  int gemm_backend = 0;   // 0 (default) = own FP64 DMMA kernels; 4 = INT8 tensor cores (wgmma s8, TMA-fed; i8emu.cu / i8tc2.cu) for
+                          // contractions of at least i8_min_rows rows, DMMA otherwise; 1 = cuBLAS (A/B comparison only); 2 = checker of
+                          // the INT8 scheme (integer products on CUDA cores).  DMMA is the default because it is the faster of the two on
+                          // an H100 SXM (400 W): LOBPCG iteration of the 128-atom Si cell (259 bands) 0.18 s vs 0.27 s, nonlocal products
+                          // 19.2 ms vs 22.3 ms, equal eigenvalues to 1e-15
   int band_chunk = 0;     // 0 = auto
   int fft_engine = 0;     // 0 = register two-pass engine where a factor pair exists, 1 = generic Stockham (applies to grids created afterwards)
   int gemm_stages = 2;    // cp.async ring depth of the DMMA GEMMs (2 -> 4 CTAs/SM, 3 -> 2 CTAs/SM)
   int64_t i8_min_rows = 32768;   // gemm_backend 4: shortest contraction length that goes to the INT8 tensor-core path
-  int z_pipeline = 0;     // fused z stage of the H apply: 0 = one tile per CTA (default), 1 = persistent cp.async-pipelined kernel (measured 6 % slower at 192^3, profiles/README.md)
+  int z_pipeline = 0;     // fused z stage of the H apply: 0 = one tile per CTA (default), 1 = persistent cp.async-pipelined kernel
   int force_svd_fallback = 0;   // test hook: the next N ortho! calls behave as if safe_cholesky had given up
   int small_dense = 1;    // LOBPCG with <= 32 bands: fused small-matrix kernels (lobpcg_small.cuh); 0 = GEMM + cuSOLVER path
   dftk::DevBuf<int> small_counter;   // arrival counter of k_small_gram (kept at zero between launches)
-  int sm_count = 148;
+  int sm_count = 132;
   std::string last_error;
   dftk::DevBuf<char> solver_work;
   dftk::DevBuf<int> dev_info;
@@ -133,8 +135,7 @@ struct dftk_b200_ctx {
   cudaStream_t batch_user_stream = nullptr;   // the context's own stream while a pipelined batch has swapped ctx->stream
   bool batch_pipelined = false;
   int batch_pipeline = 0;     // option: 1 = two pipelined groups for batches of >= 8 k-blocks, 0 (default) = one group (one sync per
-                              // round).  Measured equal within 1 % on C4 / C5 and 15 % slower on C2 (profiles/README.md): the rounds
-                              // are bound by the kernels, not by the host, so the doubled launch count buys nothing
+                              // round)
   double lobpcg_flops = 0.0;  // FP64-equivalent GEMM flops executed by the large-path LOBPCG solves (Gram, update, Cholesky-QR, nonlocal) since reset
   int64_t batch_rounds = 0;   // scheduler rounds (= host synchronisations) of the batched solves since creation / reset
 };

@@ -56,7 +56,7 @@ HD cplx twiddle(const cplx* __restrict__ tw, int m, int sign) {
   return w;
 }
 
-// One Stockham autosort pass of radix R over L lines (see DESIGN.md "1D engine").
+// One Stockham autosort pass of radix R over L lines.
 template <int R>
 HD void butterfly(cplx* v, int sign) {
   const double s = (double)sign;

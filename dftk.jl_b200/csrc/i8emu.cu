@@ -1,8 +1,6 @@
 // Reference device pipeline of the INT8-emulated FP64 complex GEMM (i8emu_core.cuh): column scales -> int8 residue planes
-// -> per-modulus integer dot products -> CRT.  Reached only through option gemm_backend = 2 (C = A^H B, alpha = 1,
-// beta = 0).  The integer products here are plain CUDA-core loops: this file is the checker and the plumbing into which a
-// `tcgen05.mma.kind::i8` kernel drops (scripts/tcgen05_i8_probe.cu is the hardware bring-up probe); it is groundwork, not
-// a measured path, and has not run on hardware yet.
+// -> per-modulus integer dot products -> CRT.  The integer products of option gemm_backend = 2 are plain CUDA-core loops
+// (the checker); gemm_backend = 4 runs them on the tensor cores (i8tc2.cu).
 #include "structs.cuh"
 #include "i8emu_core.cuh"
 
@@ -226,7 +224,7 @@ I8Operand i8_prepare(dftk_b200_ctx* ctx, const cplx* X, int64_t ld, int64_t cols
   op.exps = e;
   return op;
 }
-// C (A.cols x B.cols, leading dimension ldc) = A^H B from prepared operands: TMA-fed tcgen05.mma.kind::i8 products, chunk sums, CRT.
+// C (A.cols x B.cols, leading dimension ldc) = A^H B from prepared operands: TMA-fed wgmma s8 products, chunk sums, CRT.
 // upper_only: tiles strictly below the diagonal are skipped (their entries of C are unspecified), as in the DMMA kernel.
 void i8_gram(dftk_b200_ctx* ctx, const I8Operand& A, const I8Operand& B, cplx* C, int64_t ldc, bool upper_only) {
   REQUIRE(A.k == B.k && A.ldk == B.ldk && A.n_mod == B.n_mod, "i8_gram: operands prepared for different contraction lengths");
@@ -368,8 +366,7 @@ void i8_update(dftk_b200_ctx* ctx, int n_blocks, const I8Operand* A, const cplx*
 }
 
 void zgemm_i8_cn(dftk_b200_ctx* ctx, int64_t m, int64_t n, int64_t k, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
-                 cplx* C, int64_t ldc, int tc_mode, const signed char* ra_cached, const int* ea_cached) {
-  const bool tensor_cores = tc_mode != 0;      // 1: cp.async-fed kernel (i8tc.cu), 2: TMA-fed kernel (i8tc2.cu)
+                 cplx* C, int64_t ldc, bool tensor_cores, const signed char* ra_cached, const int* ea_cached) {
   if (m == 0 || n == 0) return;
   REQUIRE(k >= 1 && m <= 65535 && n <= 65535, "zgemm_i8: unsupported shape");
   const I8Tables T = tables_for(2 * k);
@@ -402,8 +399,7 @@ void zgemm_i8_cn(dftk_b200_ctx* ctx, int64_t m, int64_t n, int64_t k, const cplx
              T.n_mod, ra);
     LAUNCH(ctx, k_i8_residues_ld4, dim3((unsigned)((ldk / 4 + 255) / 256), (unsigned)n), 256, 0, B, ldb, k, n, ldk, (const int*)eb,
            T.n_mod, rb);
-    if (tc_mode == 2) i8tc2_products(ctx, ra, rb, m, n, ldk, T.n_mod, part, res, false);
-    else i8tc_products(ctx, ra, rb, m, n, ldk, T.n_mod, part, res);
+    i8tc2_products(ctx, ra, rb, m, n, ldk, T.n_mod, part, res, false);
   } else {
     LAUNCH(ctx, k_i8_residues, dim3((unsigned)((k + 255) / 256), (unsigned)m), 256, 0, A, lda, k, m, (const int*)ea, T.n_mod, ra);
     LAUNCH(ctx, k_i8_residues, dim3((unsigned)((k + 255) / 256), (unsigned)n), 256, 0, B, ldb, k, n, (const int*)eb, T.n_mod, rb);

@@ -1,7 +1,7 @@
-// FP64 complex GEMM emulated with INT8 products and INT32 accumulation (groundwork for moving the GEMM-shaped half of
-// H psi -- P' psi, P (D P' psi), the LOBPCG Gram/update products -- from the FP64 DMMA pipe onto the 5th-generation tensor
-// cores: `tcgen05.mma.kind::i8` multiplies s8 x s8 into s32 TMEM accumulators).  NOT on the default path (option
-// gemm_backend = 2); scripts/ozaki_study.py holds the numerics study that selected the scheme.
+// FP64 complex GEMM emulated with INT8 products and INT32 accumulation: the GEMM-shaped half of H psi -- P' psi,
+// P (D P' psi), the LOBPCG Gram/update products -- moves from the FP64 DMMA pipe onto the INT8 tensor cores (Hopper
+// `wgmma ... .s32.s8.s8` multiplies s8 x s8 into s32 register accumulators, i8tc2.cu).  scripts/ozaki_study.py holds the
+// numerics study that selected the scheme.
 //
 // Scheme (integer modular technique, Ozaki / Uchino / Imamura 2025):
 //   1. every column of an operand (a vector along the contraction index) gets a power-of-two scale 2^e such that

@@ -1,39 +1,43 @@
-// Second tensor-core kernel of the INT8-residue GEMM emulation (option gemm_backend = 4): the same products as i8tc.cu
-//     X1 = Ar^T Br,  X2 = Ai^T Bi,  X3 = Ar^T Bi,  X4 = Ai^T Br          (s8 x s8 -> s32, tcgen05.mma.kind::i8)
-// but the operand tiles travel global -> shared by TMA (`cp.async.bulk.tensor.2d`, 128-byte swizzle) instead of 4096
-// cp.async pieces per stage.  i8tc.cu measured 0.69 POPS (15 % of the issue rate of the same MMAs on resident operands):
-// its producers spend 32 cp.async + address arithmetic per thread and stage and fill the no-swizzle layout in 16-byte
-// granules.  Here one lane issues four box copies per stage (128 rows x 128 B each, full 128-byte lines) and the MMA lane
-// advances the K-major SWIZZLE_128B descriptors by 32 bytes per K = 32 step.
+// Tensor-core kernels of the INT8-residue GEMM emulation (option gemm_backend = 4, i8emu_core.cuh): for one modulus they form
+// the four integer products
+//     X1 = Ar^T Br,  X2 = Ai^T Bi,  X3 = Ar^T Bi,  X4 = Ai^T Br          (s8 x s8 -> s32, Hopper `wgmma.mma_async ... .s32.s8.s8`)
+// of the residue planes and write their residues modulo p.
 //
-//   warp 0:    TMA producer (one elected lane), mbarrier expect_tx / complete_tx per stage
-//   warp 1:    MMA issuer (one elected lane); tcgen05.commit releases stages / signals the epilogue; TMEM alloc / dealloc
-//   warps 2-5: epilogue (tcgen05.ld: TMEM lane = output row), residues modulo p of this K chunk as int16
+// Operand tiles travel global -> shared by TMA (`cp.async.bulk.tensor.2d`, 128-byte swizzle) into a ring of stages guarded
+// by mbarriers (full: TMA transaction bytes, empty: one arrival per consumer thread).  Two consumer warpgroups own 64 output
+// rows each and keep the four accumulators in registers; one producer warp issues the copies.  A consumer keeps one wgmma
+// group in flight (wait_group 1) and releases a stage once the group that read it has completed.
 //
-// Shared-memory descriptor (cute::UMMA::SmemDescriptor, K-major, SWIZZLE_128B, cf. cute/atom/mma_traits_sm100.hpp): canonical
-// layout ((8,n),2):((8,SBO),1) in 16-byte units -> rows 128 B apart, LBO = 1, SBO = 1024 B (eight rows), layout type 2,
-// version 1; the tile base is 1024-byte aligned (the swizzle XORs address bits [4,7) with bits [7,10)).
+// Shared-memory descriptor (sm_90 GMMA descriptor, K-major, SWIZZLE_128B): start address, LBO unused (one swizzle atom covers
+// the 32-byte K extent of one instruction), SBO = 1024 B between 8-row groups, layout type 1.  Rows are 128 bytes of K; a
+// K = 32 step advances the start address by 32 bytes.  Tile bases are 1024-byte aligned (the swizzle XORs address bits
+// [4,7) with bits [7,10)).  wgmma takes 8-bit operands K-major only, so the update-type kernel transposes its MN-major tall
+// operand in shared memory before the MMAs.
 #include <cuda.h>
 #include <algorithm>
 #include <string>
-#include <vector>
 #include "structs.cuh"
 #include "i8emu_core.cuh"
 
 namespace dftk {
 
-constexpr int T2_M = 128;        // output rows per tile (TMEM lanes)
-constexpr int T2_N = 128;        // output columns per tile (4 accumulators x 128 columns = 512 TMEM columns)
+constexpr int T2_M = 128;        // output rows per tile: two warpgroups x 64
+constexpr int T2_N = 64;         // output columns per tile (4 accumulators x 32 registers per thread)
 constexpr int T2_BK = 128;       // K bytes per stage = one swizzle row
-constexpr int T2_STAGES = 3;
-constexpr int T2_TILE_BYTES = T2_M * T2_BK;                      // 16 KB
-constexpr int T2_STAGE_BYTES = 4 * T2_TILE_BYTES;                // Ar, Ai, Br, Bi
+constexpr int T2_STAGES = 4;
+constexpr int T2_A_BYTES = T2_M * T2_BK;                         // 16 KB
+constexpr int T2_B_BYTES = T2_N * T2_BK;                         // 8 KB
+constexpr int T2_STAGE_BYTES = 2 * T2_A_BYTES + 2 * T2_B_BYTES;  // Ar, Ai, Br, Bi
 constexpr int T2_SMEM = T2_STAGES * T2_STAGE_BYTES + 1024;       // + alignment slack
-constexpr int T2_THREADS = 192;
+constexpr int T2_THREADS = 288;                                  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int T2_CONSUMERS = 256;
 
 __device__ __forceinline__ uint32_t t2_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void t2_mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(t2_smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void t2_mbar_arrive(uint64_t* bar) {
+  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" :: "r"(t2_smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void t2_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" :: "r"(t2_smem_u32(bar)), "r"(bytes) : "memory");
@@ -51,44 +55,44 @@ __device__ __forceinline__ void t2_mbar_wait(uint64_t* bar, uint32_t parity) {
     if (clock64() - t0 > 4000000000ll) __trap();
   }
 }
-__device__ __forceinline__ void t2_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(t2_smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void t2_tma_load(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       :: "r"(t2_smem_u32(smem_dst)), "l"(map), "r"(c0), "r"(c1), "r"(t2_smem_u32(bar)) : "memory");
 }
-// K-major SWIZZLE_128B operand descriptor: start address, LBO = 16 B (unused for one swizzle atom in K), SBO = 1024 B
+// K-major SWIZZLE_128B operand descriptor (LBO = 16 B, unused; SBO = 1024 B; layout type 1 = 128-byte swizzle)
 __device__ __forceinline__ uint64_t t2_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-__device__ __forceinline__ void t2_mma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void t2_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void t2_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void t2_wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void t2_wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// d (64 x 64 s32, warpgroup fragment) += A (64 x 32 s8) B (32 x 64 s8), both from shared memory
+__device__ __forceinline__ void t2_mma(int (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}\n"
-      :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]),
+        "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]),
+        "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]),
+        "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "l"(da), "l"(db));
 }
-__device__ __forceinline__ void t2_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
+// accumulator fragment of m64nNk32: register r of thread (warp w of the warpgroup, lane l) holds row w*16 + l/4 + 8*((r/2)%2)
+// and column (r/4)*8 + 2*(l%4) + r%2
+__device__ __forceinline__ int t2_frag_row(int r, int wq, int lane) { return wq * 16 + (lane >> 2) + 8 * ((r >> 1) & 1); }
+__device__ __forceinline__ int t2_frag_col(int r, int lane) { return (r >> 2) * 8 + 2 * (lane & 3) + (r & 1); }
 
-// tensor maps: 2-D views [rows_total][ldk] of the residue planes of A (2 n_mod m rows) and B (2 n_mod n rows), box 128 x 128 B.
-// grid (m tiles, n tiles, n_mod * n_chunks).  part[(chunk)][(2 t + part)][j][i] int16 as in i8tc.cu.
+// tensor maps: 2-D views [rows_total][ldk] of the residue planes of A (2 n_mod m rows, box 128 rows) and B (2 n_mod n rows,
+// box 64 rows), 128 bytes of K per box.  grid (m tiles, n tiles, n_mod * n_chunks).  part[(chunk)][(2 t + part)][j][i] int16.
 __global__ void __launch_bounds__(T2_THREADS, 1)
 k_i8_gemm_tc2(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int64_t m, int64_t n,
               int64_t ldk, int n_mod, int n_chunks, int64_t chunk_len, short* __restrict__ part, int upper_only) {
@@ -96,12 +100,9 @@ k_i8_gemm_tc2(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
   if (upper_only && (int64_t)blockIdx.x * T2_M >= (int64_t)blockIdx.y * T2_N + T2_N) return;
   extern __shared__ unsigned char t2_raw[];
   unsigned char* sm = (unsigned char*)(((uintptr_t)t2_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[T2_STAGES], empty_bar[T2_STAGES], accum_bar;
-  __shared__ uint32_t tmem_base;
+  __shared__ __align__(8) uint64_t full_bar[T2_STAGES], empty_bar[T2_STAGES];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int t = blockIdx.z % n_mod, chunk = blockIdx.z / n_mod;
-  const int p = i8_modulus(t);
-  const unsigned long long magic = i8_barrett_magic(p);
   const int64_t i0 = (int64_t)blockIdx.x * T2_M, j0 = (int64_t)blockIdx.y * T2_N;
   const int64_t k_begin = (int64_t)chunk * chunk_len;
   const int64_t k_end = k_begin + chunk_len < ldk ? k_begin + chunk_len : ldk;
@@ -109,22 +110,14 @@ k_i8_gemm_tc2(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
 
   if (tid == 0) {
     for (int s = 0; s < T2_STAGES; ++s) {
-      t2_mbar_init(&full_bar[s], 1);         // one arrive.expect_tx by the producer lane (+ the TMA transaction bytes)
-      t2_mbar_init(&empty_bar[s], 1);        // one tcgen05.commit
+      t2_mbar_init(&full_bar[s], 1);                 // one arrive.expect_tx by the producer lane (+ the TMA transaction bytes)
+      t2_mbar_init(&empty_bar[s], T2_CONSUMERS);     // every consumer thread once its MMAs of the stage have completed
     }
-    t2_mbar_init(&accum_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(t2_smem_u32(&tmem_base)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ---------------- TMA producer
     if (lane == 0) {
       const int row_ar = (int)((int64_t)(2 * t) * m + i0), row_ai = (int)((int64_t)(2 * t + 1) * m + i0);
@@ -135,85 +128,70 @@ k_i8_gemm_tc2(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
         unsigned char* stage = sm + (size_t)s * T2_STAGE_BYTES;
         const int kc = (int)(k_begin + (int64_t)it * T2_BK);
         t2_mbar_expect_tx(&full_bar[s], (uint32_t)T2_STAGE_BYTES);
-        t2_tma_load(stage + 0 * T2_TILE_BYTES, &map_a, kc, row_ar, &full_bar[s]);
-        t2_tma_load(stage + 1 * T2_TILE_BYTES, &map_a, kc, row_ai, &full_bar[s]);
-        t2_tma_load(stage + 2 * T2_TILE_BYTES, &map_b, kc, row_br, &full_bar[s]);
-        t2_tma_load(stage + 3 * T2_TILE_BYTES, &map_b, kc, row_bi, &full_bar[s]);
+        t2_tma_load(stage, &map_a, kc, row_ar, &full_bar[s]);
+        t2_tma_load(stage + T2_A_BYTES, &map_a, kc, row_ai, &full_bar[s]);
+        t2_tma_load(stage + 2 * T2_A_BYTES, &map_b, kc, row_br, &full_bar[s]);
+        t2_tma_load(stage + 2 * T2_A_BYTES + T2_B_BYTES, &map_b, kc, row_bi, &full_bar[s]);
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer
-    // instruction descriptor: D = s32, A = B = s8, both K-major, N = 128, M = 128  (cute::UMMA::InstrDescriptor)
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(T2_N >> 3) << 17) | ((uint32_t)(T2_M >> 4) << 24);
-    for (int it = 0; it < n_iters; ++it) {
-      const int s = it % T2_STAGES;
-      t2_mbar_wait(&full_bar[s], (uint32_t)((it / T2_STAGES) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t base = t2_smem_u32(sm + (size_t)s * T2_STAGE_BYTES);
+    return;
+  }
+  // ---------------- consumers: warpgroup g = rows [64 g, 64 g + 64) of the tile
+  const int g = warp >> 2, wq = warp & 3;
+  int x1[32], x2[32], x3[32], x4[32];
 #pragma unroll
-        for (int kk = 0; kk < T2_BK / 32; ++kk) {
-          const uint32_t koff = (uint32_t)kk * 32u;                 // 32 bytes of K per MMA inside the 128-byte swizzle row
-          const uint64_t dAr = t2_desc(base + 0 * T2_TILE_BYTES + koff);
-          const uint64_t dAi = t2_desc(base + 1 * T2_TILE_BYTES + koff);
-          const uint64_t dBr = t2_desc(base + 2 * T2_TILE_BYTES + koff);
-          const uint64_t dBi = t2_desc(base + 3 * T2_TILE_BYTES + koff);
-          const uint32_t acc = (uint32_t)(it > 0 || kk > 0);
-          t2_mma_i8(tmem + 0 * T2_N, dAr, dBr, idesc, acc);
-          t2_mma_i8(tmem + 1 * T2_N, dAi, dBi, idesc, acc);
-          t2_mma_i8(tmem + 2 * T2_N, dAr, dBi, idesc, acc);
-          t2_mma_i8(tmem + 3 * T2_N, dAi, dBr, idesc, acc);
-        }
-        t2_commit(&empty_bar[s]);                    // frees the stage once these MMAs have read it
-        if (it == n_iters - 1) t2_commit(&accum_bar);
-      }
-      __syncwarp();
+  for (int r = 0; r < 32; ++r) x1[r] = x2[r] = x3[r] = x4[r] = 0;
+  for (int it = 0; it < n_iters; ++it) {
+    const int s = it % T2_STAGES;
+    t2_mbar_wait(&full_bar[s], (uint32_t)((it / T2_STAGES) & 1));
+    const uint32_t base = t2_smem_u32(sm + (size_t)s * T2_STAGE_BYTES);
+    const uint32_t ar = base + g * (64 * T2_BK), ai = ar + T2_A_BYTES;
+    const uint32_t br = base + 2 * T2_A_BYTES, bi = br + T2_B_BYTES;
+    t2_wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < T2_BK / 32; ++kk) {
+      const uint32_t ko = (uint32_t)kk * 32u;
+      t2_mma(x1, t2_desc(ar + ko), t2_desc(br + ko));
+      t2_mma(x2, t2_desc(ai + ko), t2_desc(bi + ko));
+      t2_mma(x3, t2_desc(ar + ko), t2_desc(bi + ko));
+      t2_mma(x4, t2_desc(ai + ko), t2_desc(br + ko));
     }
-  } else {
-    // ---------------- epilogue: warps 2..5 own the TMEM lane quarters (warp % 4); thread = output row
-    t2_mbar_wait(&accum_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int quarter = warp & 3;
-    const int64_t i = i0 + quarter * 32 + lane;
-    short* out_re = part + (((size_t)chunk * 2 * n_mod + 2 * t) * n) * m;
-    short* out_im = part + (((size_t)chunk * 2 * n_mod + 2 * t + 1) * n) * m;
-    for (int c0 = 0; c0 < T2_N; c0 += 32) {
-      uint32_t x1[32], x2[32], x3[32], x4[32];
-      const uint32_t lane_base = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0;
-      t2_ld32(lane_base + 0 * T2_N, x1);
-      t2_ld32(lane_base + 1 * T2_N, x2);
-      t2_ld32(lane_base + 2 * T2_N, x3);
-      t2_ld32(lane_base + 3 * T2_N, x4);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (i < m) {
+    t2_wgmma_commit();
+    t2_wgmma_wait1();                                                    // the group of it - 1 has completed
+    if (it > 0) t2_mbar_arrive(&empty_bar[(it - 1) % T2_STAGES]);        // its stage is free
+  }
+  t2_wgmma_wait0();
+  // ---------------- epilogue: residues modulo p of this K chunk as int16
+  const int p = i8_modulus(t);
+  const unsigned long long magic = i8_barrett_magic(p);
+  short* out_re = part + (((size_t)chunk * 2 * n_mod + 2 * t) * n) * m;
+  short* out_im = part + (((size_t)chunk * 2 * n_mod + 2 * t + 1) * n) * m;
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const int64_t j = j0 + c0 + c;
-          if (j < n) {
-            // |x| <= 2^16 x 2^14: reduce each accumulator first (the sum of two would overflow int32)
-            const int re = i8_reduce_sym(i8_reduce_sym((int)x1[c] >> 4, p, magic) * 16 + ((int)x1[c] & 15) +
-                                         i8_reduce_sym((int)x2[c] >> 4, p, magic) * 16 + ((int)x2[c] & 15), p, magic);
-            const int im = i8_reduce_sym(i8_reduce_sym((int)x3[c] >> 4, p, magic) * 16 + ((int)x3[c] & 15) -
-                                         i8_reduce_sym((int)x4[c] >> 4, p, magic) * 16 - ((int)x4[c] & 15), p, magic);
-            out_re[(size_t)j * m + i] = (short)re;
-            out_im[(size_t)j * m + i] = (short)im;
-          }
-        }
-      }
+  for (int r = 0; r < 32; ++r) {
+    const int64_t i = i0 + g * 64 + t2_frag_row(r, wq, lane), j = j0 + t2_frag_col(r, lane);
+    if (i < m && j < n) {
+      // |x| <= 2^16 x 2^14: reduce each accumulator first (the sum of two would overflow int32)
+      const int re = i8_reduce_sym(i8_reduce_sym(x1[r] >> 4, p, magic) * 16 + (x1[r] & 15) +
+                                   i8_reduce_sym(x2[r] >> 4, p, magic) * 16 + (x2[r] & 15), p, magic);
+      const int im = i8_reduce_sym(i8_reduce_sym(x3[r] >> 4, p, magic) * 16 + (x3[r] & 15) -
+                                   i8_reduce_sym(x4[r] >> 4, p, magic) * 16 - (x4[r] & 15), p, magic);
+      out_re[(size_t)j * m + i] = (short)re;
+      out_im[(size_t)j * m + i] = (short)im;
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(512) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
 // Update-type products  C (m x n) = sum over blocks  A_b (m x K_b) B_b (K_b x n)  (LazyHcat * matrix of LOBPCG, P (D P'psi)):
-// the tall operand A_b is consumed in its stored orientation as the MN-major UMMA operand -- its residue planes
-// [plane][column k][row G] are the ones the Gram products already prepared (G contiguous) -- and the small matrix B as the
-// K-major operand.  Complex product without conjugation: re = X1 - X2, im = X3 + X4.  All blocks accumulate in TMEM
-// (|sum| <= 1536 x 2^14: no int32 overflow); the epilogue writes the symmetric residues as int8.
-// grid (n tiles, m tiles, n_mod): the n tiles of one G tile are neighbours in launch order and share the A tile in L2.
+// the tall operand A_b arrives in its stored orientation -- its residue planes [plane][column k][row G] are the ones the Gram
+// products already prepared (G contiguous) -- and the small matrix B as K-major planes [plane][j][k].  Complex product
+// without conjugation: re = X1 - X2, im = X3 + X4.  All blocks accumulate in registers (|sum| <= 1536 x 2^14: no int32
+// overflow); the epilogue writes the symmetric residues as int8.
+// The product is formed transposed, D[j, G] = sum_k B~[k, j] A[G, k]: the small matrix is the wgmma "A" operand (64 rows j
+// per warpgroup), the tall operand the "B" operand (64 columns G).  Its stage holds the MN-major box [128 k][64 G]; the
+// consumer threads transpose it into the K-major swizzled layout [64 G][128 k] (4 x 4 byte blocks through byte permutes)
+// before the MMAs read it.  grid (n tiles, m tiles, n_mod): the n tiles of one G tile are neighbours in launch order and
+// share the A tile in L2.
 struct T2NnBlocks {
   int n_blocks;
   int kcols[3];      // columns of A_b = rows of its planes
@@ -221,46 +199,61 @@ struct T2NnBlocks {
   int k_off[3];      // first (padded) contraction index of the block in B's planes (multiple of 128)
 };
 
-constexpr int T2NN_THREADS = 320;    // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two warps per TMEM lane quarter)
+constexpr int NN_STAGES = 3;
+constexpr int NN_S_BYTES = T2_M * T2_BK;                           // small matrix: 128 rows j x 128 k (16 KB)
+constexpr int NN_T_BYTES = T2_BK * T2_N;                           // tall operand: 128 k x 64 G (8 KB), both orientations
+constexpr int NN_STAGE_BYTES = 2 * NN_S_BYTES + 2 * NN_T_BYTES;   // Sr, Si, Tr, Ti (MN-major)
+constexpr int NN_TT_BUFS = 3;                                      // transposed [Tr | Ti] tiles (one MMA group in flight)
+constexpr int NN_SMEM = NN_STAGES * NN_STAGE_BYTES + NN_TT_BUFS * 2 * NN_T_BYTES + 1024;
 
-// The product is formed transposed, D[j, G] = sum_k B~[k, j] A[G, k]: the small matrix is the K-major "A" operand of the MMA
-// (128 rows j), the tall operand the MN-major "B" operand (128 columns G).  A TMEM lane then holds one row j of the output and
-// 32 consecutive G per tcgen05.ld: the residues leave as 16-byte stores (the straightforward orientation needed one byte store
-// per value and was bound by its epilogue: ncu 15 % tensor-pipe active, 4.7e9 instructions).
-__global__ void __launch_bounds__(T2NN_THREADS, 1)
+// [128 k][64 G] (row-major) -> [64 G][128 k] in the 128-byte swizzle; 256 consumer threads, both parts
+__device__ __forceinline__ void t2_transpose(const unsigned char* src, unsigned char* dst, int tid) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int b = tid + T2_CONSUMERS * q;              // 1024 blocks of 4 x 4 bytes: part, 32 k blocks, 16 G blocks
+    const int part = b >> 9, kb = (b >> 4) & 31, gb = b & 15;
+    const unsigned char* s = src + part * NN_T_BYTES + (4 * kb) * T2_N + 4 * gb;
+    const uint32_t w0 = *reinterpret_cast<const uint32_t*>(s);
+    const uint32_t w1 = *reinterpret_cast<const uint32_t*>(s + T2_N);
+    const uint32_t w2 = *reinterpret_cast<const uint32_t*>(s + 2 * T2_N);
+    const uint32_t w3 = *reinterpret_cast<const uint32_t*>(s + 3 * T2_N);
+    const uint32_t t0 = __byte_perm(w0, w1, 0x5140), t1 = __byte_perm(w2, w3, 0x5140);
+    const uint32_t t2 = __byte_perm(w0, w1, 0x7362), t3 = __byte_perm(w2, w3, 0x7362);
+    const uint32_t o[4] = {__byte_perm(t0, t1, 0x5410), __byte_perm(t0, t1, 0x7632), __byte_perm(t2, t3, 0x5410),
+                           __byte_perm(t2, t3, 0x7632)};
+    unsigned char* d = dst + part * NN_T_BYTES;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int G = 4 * gb + c;                        // o[c]: k = 4 kb .. 4 kb + 3 of column G
+      *reinterpret_cast<uint32_t*>(d + G * T2_BK + ((((kb >> 2) ^ (G & 7)) << 4) | ((4 * kb) & 15))) = o[c];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(T2_THREADS, 1)
 k_i8_gemm_tc2_nn(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                  const __grid_constant__ CUtensorMap map_a2, const __grid_constant__ CUtensorMap map_b, T2NnBlocks blocks,
                  int64_t m, int64_t n, int n_mod, signed char* __restrict__ resid, int64_t ldm) {
   extern __shared__ unsigned char t2_raw[];
   unsigned char* sm = (unsigned char*)(((uintptr_t)t2_raw + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[T2_STAGES], empty_bar[T2_STAGES], accum_bar;
-  __shared__ uint32_t tmem_base;
+  unsigned char* tt = sm + NN_STAGES * NN_STAGE_BYTES;               // transposed tall tiles, NN_TT_BUFS buffers
+  __shared__ __align__(8) uint64_t full_bar[NN_STAGES], empty_bar[NN_STAGES];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int t = blockIdx.z;
-  const int p = i8_modulus(t);
-  const unsigned long long magic = i8_barrett_magic(p);
   const int64_t j0 = (int64_t)blockIdx.x * T2_M, i0 = (int64_t)blockIdx.y * T2_N;      // j: MMA rows, G: MMA columns
   int total_iters = 0;
   for (int b = 0; b < blocks.n_blocks; ++b) total_iters += blocks.n_iters[b];
 
   if (tid == 0) {
-    for (int s = 0; s < T2_STAGES; ++s) {
+    for (int s = 0; s < NN_STAGES; ++s) {
       t2_mbar_init(&full_bar[s], 1);
-      t2_mbar_init(&empty_bar[s], 1);
+      t2_mbar_init(&empty_bar[s], T2_CONSUMERS);
     }
-    t2_mbar_init(&accum_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(t2_smem_u32(&tmem_base)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       const int row_br = (int)((int64_t)(2 * t) * n + j0), row_bi = (int)((int64_t)(2 * t + 1) * n + j0);
       int it = 0;
@@ -268,88 +261,68 @@ k_i8_gemm_tc2_nn(const __grid_constant__ CUtensorMap map_a0, const __grid_consta
         const CUtensorMap* ma = b == 0 ? &map_a0 : (b == 1 ? &map_a1 : &map_a2);
         const int kc = blocks.kcols[b];
         for (int q = 0; q < blocks.n_iters[b]; ++q, ++it) {
-          const int s = it % T2_STAGES;
-          if (it >= T2_STAGES) t2_mbar_wait(&empty_bar[s], (uint32_t)((it / T2_STAGES - 1) & 1));
-          unsigned char* stage = sm + (size_t)s * T2_STAGE_BYTES;
-          t2_mbar_expect_tx(&full_bar[s], (uint32_t)T2_STAGE_BYTES);
-          // tall operand: 128 contraction rows (plane rows k) x 128 bytes of G; small matrix: 128 rows j x 128 bytes of k
-          t2_tma_load(stage + 0 * T2_TILE_BYTES, ma, (int)i0, (2 * t) * kc + q * T2_BK, &full_bar[s]);
-          t2_tma_load(stage + 1 * T2_TILE_BYTES, ma, (int)i0, (2 * t + 1) * kc + q * T2_BK, &full_bar[s]);
-          t2_tma_load(stage + 2 * T2_TILE_BYTES, &map_b, blocks.k_off[b] + q * T2_BK, row_br, &full_bar[s]);
-          t2_tma_load(stage + 3 * T2_TILE_BYTES, &map_b, blocks.k_off[b] + q * T2_BK, row_bi, &full_bar[s]);
+          const int s = it % NN_STAGES;
+          if (it >= NN_STAGES) t2_mbar_wait(&empty_bar[s], (uint32_t)((it / NN_STAGES - 1) & 1));
+          unsigned char* stage = sm + (size_t)s * NN_STAGE_BYTES;
+          t2_mbar_expect_tx(&full_bar[s], (uint32_t)NN_STAGE_BYTES);
+          // small matrix: 128 rows j x 128 bytes of k; tall operand: 128 contraction rows (plane rows k) x 64 bytes of G
+          t2_tma_load(stage, &map_b, blocks.k_off[b] + q * T2_BK, row_br, &full_bar[s]);
+          t2_tma_load(stage + NN_S_BYTES, &map_b, blocks.k_off[b] + q * T2_BK, row_bi, &full_bar[s]);
+          t2_tma_load(stage + 2 * NN_S_BYTES, ma, (int)i0, (2 * t) * kc + q * T2_BK, &full_bar[s]);
+          t2_tma_load(stage + 2 * NN_S_BYTES + NN_T_BYTES, ma, (int)i0, (2 * t + 1) * kc + q * T2_BK, &full_bar[s]);
         }
       }
     }
-  } else if (warp == 1) {
-    // D = s32, A = B = s8; MMA-A (small matrix) K-major, MMA-B (tall operand) MN-major (bit 16); N = 128, M = 128
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((uint32_t)(T2_N >> 3) << 17) | ((uint32_t)(T2_M >> 4) << 24);
-    for (int it = 0; it < total_iters; ++it) {
-      const int s = it % T2_STAGES;
-      t2_mbar_wait(&full_bar[s], (uint32_t)((it / T2_STAGES) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t base = t2_smem_u32(sm + (size_t)s * T2_STAGE_BYTES);
+    return;
+  }
+  const int g = warp >> 2, wq = warp & 3;
+  int x1[32], x2[32], x3[32], x4[32];
 #pragma unroll
-        for (int kk = 0; kk < T2_BK / 32; ++kk) {
-          // tall operand (MN-major, SWIZZLE_128B): a K = 32 step is 32 rows of 128 bytes = 4096 bytes; small matrix (K-major): 32 bytes
-          const uint64_t dTr = t2_desc(base + 0 * T2_TILE_BYTES + (uint32_t)kk * 4096u);
-          const uint64_t dTi = t2_desc(base + 1 * T2_TILE_BYTES + (uint32_t)kk * 4096u);
-          const uint64_t dSr = t2_desc(base + 2 * T2_TILE_BYTES + (uint32_t)kk * 32u);
-          const uint64_t dSi = t2_desc(base + 3 * T2_TILE_BYTES + (uint32_t)kk * 32u);
-          const uint32_t acc = (uint32_t)(it > 0 || kk > 0);
-          t2_mma_i8(tmem + 0 * T2_N, dSr, dTr, idesc, acc);      // X1 = Sr Tr
-          t2_mma_i8(tmem + 1 * T2_N, dSi, dTi, idesc, acc);      // X2 = Si Ti
-          t2_mma_i8(tmem + 2 * T2_N, dSi, dTr, idesc, acc);      // X3 = Si Tr   (tall re x small im)
-          t2_mma_i8(tmem + 3 * T2_N, dSr, dTi, idesc, acc);      // X4 = Sr Ti   (tall im x small re)
-        }
-        t2_commit(&empty_bar[s]);
-        if (it == total_iters - 1) t2_commit(&accum_bar);
-      }
-      __syncwarp();
+  for (int r = 0; r < 32; ++r) x1[r] = x2[r] = x3[r] = x4[r] = 0;
+  for (int it = 0; it < total_iters; ++it) {
+    const int s = it % NN_STAGES;
+    t2_mbar_wait(&full_bar[s], (uint32_t)((it / NN_STAGES) & 1));
+    unsigned char* stage = sm + (size_t)s * NN_STAGE_BYTES;
+    unsigned char* tb = tt + (it % NN_TT_BUFS) * 2 * NN_T_BYTES;
+    // buffer it % 3 was last read by the MMAs of iteration it - 3; every consumer waited for them (wait_group 1 at the end of
+    // iteration it - 2) before it arrived at the barrier of iteration it - 1
+    t2_transpose(stage + 2 * NN_S_BYTES, tb, tid);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> visible to wgmma
+    asm volatile("bar.sync 1, %0;" :: "n"(T2_CONSUMERS) : "memory");
+    const uint32_t sr = t2_smem_u32(stage) + g * (64 * T2_BK), si = sr + NN_S_BYTES;
+    const uint32_t tr = t2_smem_u32(tb), ti = tr + NN_T_BYTES;
+    t2_wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < T2_BK / 32; ++kk) {
+      const uint32_t ko = (uint32_t)kk * 32u;
+      t2_mma(x1, t2_desc(sr + ko), t2_desc(tr + ko));      // X1 = Sr Tr
+      t2_mma(x2, t2_desc(si + ko), t2_desc(ti + ko));      // X2 = Si Ti
+      t2_mma(x3, t2_desc(si + ko), t2_desc(tr + ko));      // X3 = Si Tr   (tall re x small im)
+      t2_mma(x4, t2_desc(sr + ko), t2_desc(ti + ko));      // X4 = Sr Ti   (tall im x small re)
     }
-  } else {
-    // ---------------- epilogue: lane = row j; warps 2..9 = (quarter = warp % 4, half of the 128 G columns = (warp - 2) / 4)
-    t2_mbar_wait(&accum_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int quarter = warp & 3, half = (warp - 2) >> 2;
-    const int64_t j = j0 + quarter * 32 + lane;
-    signed char* out_re = resid + ((size_t)(2 * t) * n + (j < n ? j : 0)) * ldm + i0;
-    signed char* out_im = resid + ((size_t)(2 * t + 1) * n + (j < n ? j : 0)) * ldm + i0;
-    for (int c0 = 64 * half; c0 < 64 * half + 64; c0 += 32) {
-      uint32_t x1[32], x2[32], x3[32], x4[32];
-      const uint32_t lane_base = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0;
-      t2_ld32(lane_base + 0 * T2_N, x1);
-      t2_ld32(lane_base + 1 * T2_N, x2);
-      t2_ld32(lane_base + 2 * T2_N, x3);
-      t2_ld32(lane_base + 3 * T2_N, x4);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (j < n) {
-        // |x| <= 1536 x 2^14 < 2^25: sums and differences of two accumulators stay below 2^26
-        uint32_t wre[8], wim[8];
+    t2_wgmma_commit();
+    t2_wgmma_wait1();
+    if (it > 0) t2_mbar_arrive(&empty_bar[(it - 1) % NN_STAGES]);
+  }
+  t2_wgmma_wait0();
+  // ---------------- epilogue: pairs of consecutive G of one row j leave as 16-bit stores
+  const int p = i8_modulus(t);
+  const unsigned long long magic = i8_barrett_magic(p);
 #pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          uint32_t a = 0, b = 0;
+  for (int r = 0; r < 32; r += 2) {
+    const int64_t j = j0 + g * 64 + t2_frag_row(r, wq, lane), G = i0 + t2_frag_col(r, lane);
+    if (j < n) {
+      // |x| <= 1536 x 2^14 < 2^25: sums and differences of two accumulators stay below 2^26
+      uint32_t wre = 0, wim = 0;
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            a |= (uint32_t)(i8_reduce_sym((int)x1[c + q] - (int)x2[c + q], p, magic) & 0xFF) << (8 * q);
-            b |= (uint32_t)(i8_reduce_sym((int)x3[c + q] + (int)x4[c + q], p, magic) & 0xFF) << (8 * q);
-          }
-          wre[c >> 2] = a;
-          wim[c >> 2] = b;
-        }
-        // 32 consecutive G of row j: two 16-byte stores per part (ldm and i0 are multiples of 128: aligned)
-        uint4* pr = reinterpret_cast<uint4*>(out_re + c0);
-        uint4* pi = reinterpret_cast<uint4*>(out_im + c0);
-        pr[0] = make_uint4(wre[0], wre[1], wre[2], wre[3]);
-        pr[1] = make_uint4(wre[4], wre[5], wre[6], wre[7]);
-        pi[0] = make_uint4(wim[0], wim[1], wim[2], wim[3]);
-        pi[1] = make_uint4(wim[4], wim[5], wim[6], wim[7]);
+      for (int q = 0; q < 2; ++q) {
+        wre |= (uint32_t)(i8_reduce_sym(x1[r + q] - x2[r + q], p, magic) & 0xFF) << (8 * q);
+        wim |= (uint32_t)(i8_reduce_sym(x3[r + q] + x4[r + q], p, magic) & 0xFF) << (8 * q);
       }
+      *reinterpret_cast<uint16_t*>(resid + ((size_t)(2 * t) * n + j) * ldm + G) = (uint16_t)wre;
+      *reinterpret_cast<uint16_t*>(resid + ((size_t)(2 * t + 1) * n + j) * ldm + G) = (uint16_t)wim;
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(512) : "memory");
 }
 
 __global__ void k_i8_sum_chunks2(const short* __restrict__ part, int n_chunks, int n_mod, int64_t mn, int* __restrict__ res) {
@@ -363,8 +336,8 @@ __global__ void k_i8_sum_chunks2(const short* __restrict__ part, int n_chunks, i
 }
 
 void i8tc2_set_attributes() {
-  if (cudaFuncSetAttribute(k_i8_gemm_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM) != cudaSuccess) cudaGetLastError();
-  if (cudaFuncSetAttribute(k_i8_gemm_tc2_nn, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM) != cudaSuccess) cudaGetLastError();
+  CUDA_CHECK(cudaFuncSetAttribute(k_i8_gemm_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM));
+  CUDA_CHECK(cudaFuncSetAttribute(k_i8_gemm_tc2_nn, cudaFuncAttributeMaxDynamicSharedMemorySize, NN_SMEM));
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -381,7 +354,21 @@ static EncodeTiledFn encode_tiled() {
   }
   return fn;
 }
-static CUtensorMap plane_map(const signed char* base, int64_t rows_total, int64_t ldk);
+// 2-D view [rows_total][ld] of int8 planes; box = box_cols bytes x box_rows rows
+static CUtensorMap plane_map(const signed char* base, int64_t rows_total, int64_t ld, int box_cols, int box_rows,
+                             CUtensorMapSwizzle swizzle) {
+  CUtensorMap map;
+  const cuuint64_t gdim[2] = {(cuuint64_t)ld, (cuuint64_t)rows_total};
+  const cuuint64_t gstride[1] = {(cuuint64_t)ld};                    // bytes between rows
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  const cuuint32_t estride[2] = {1, 1};
+  const CUresult r = encode_tiled()(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)base, gdim, gstride, box, estride,
+                                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) throw Error(DFTK_B200_ECUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
+  return map;
+}
+
 // integer stage of the update-type product: blocks of prepared tall operands (planes [plane][col][ldm], ldm = padded rows) against
 // the planes of the small matrix rb ([plane][j][ldkb], contraction index padded per block); resid: int8 [(2 t + part)][j][ldm]
 void i8tc2_products_nn(dftk_b200_ctx* ctx, int n_blocks, const signed char* const* ra, const int* kcols, const int* k_off,
@@ -395,27 +382,14 @@ void i8tc2_products_nn(dftk_b200_ctx* ctx, int n_blocks, const signed char* cons
     bl.kcols[b] = kcols[b];
     bl.n_iters[b] = (kcols[b] + T2_BK - 1) / T2_BK;
     bl.k_off[b] = k_off[b];
-    maps[b] = plane_map(ra[b], 2 * (int64_t)n_mod * kcols[b], ldm);
+    maps[b] = plane_map(ra[b], 2 * (int64_t)n_mod * kcols[b], ldm, T2_N, T2_BK, CU_TENSOR_MAP_SWIZZLE_NONE);
   }
   for (int b = n_blocks; b < 3; ++b) maps[b] = maps[0];
-  const CUtensorMap map_b = plane_map(rb, 2 * (int64_t)n_mod * n, ldkb);
-  const int64_t m_tiles = (m + T2_M - 1) / T2_M;
+  const CUtensorMap map_b = plane_map(rb, 2 * (int64_t)n_mod * n, ldkb, T2_BK, T2_M, CU_TENSOR_MAP_SWIZZLE_128B);
+  const int64_t m_tiles = (m + T2_N - 1) / T2_N;
   REQUIRE(m_tiles <= 65535, "i8tc2_nn: too many row tiles");
-  dim3 grid((unsigned)((n + T2_N - 1) / T2_N), (unsigned)m_tiles, (unsigned)n_mod);
-  LAUNCH(ctx, k_i8_gemm_tc2_nn, grid, T2NN_THREADS, T2_SMEM, maps[0], maps[1], maps[2], map_b, bl, m, n, n_mod, resid, ldm);
-}
-
-static CUtensorMap plane_map(const signed char* base, int64_t rows_total, int64_t ldk) {
-  CUtensorMap map;
-  const cuuint64_t gdim[2] = {(cuuint64_t)ldk, (cuuint64_t)rows_total};
-  const cuuint64_t gstride[1] = {(cuuint64_t)ldk};                   // bytes between rows
-  const cuuint32_t box[2] = {(cuuint32_t)T2_BK, (cuuint32_t)T2_M};
-  const cuuint32_t estride[2] = {1, 1};
-  const CUresult r = encode_tiled()(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, (void*)base, gdim, gstride, box, estride,
-                                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw Error(DFTK_B200_ECUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
-  return map;
+  dim3 grid((unsigned)((n + T2_M - 1) / T2_M), (unsigned)m_tiles, (unsigned)n_mod);
+  LAUNCH(ctx, k_i8_gemm_tc2_nn, grid, T2_THREADS, NN_SMEM, maps[0], maps[1], maps[2], map_b, bl, m, n, n_mod, resid, ldm);
 }
 
 // integer stage of C = A^H B on the tensor cores, TMA-fed; ra / rb: padded residue planes (16-byte aligned, ldk % 128 == 0)
@@ -425,8 +399,8 @@ void i8tc2_products(dftk_b200_ctx* ctx, const signed char* ra, const signed char
   REQUIRE(2 * (int64_t)n_mod * std::max(m, n) < 2147483647, "i8tc2: too many plane rows");
   const int64_t chunk_len = I8_K_CHUNK;                         // multiple of T2_BK
   const int n_chunks = (int)((ldk + chunk_len - 1) / chunk_len);
-  const CUtensorMap map_a = plane_map(ra, 2 * (int64_t)n_mod * m, ldk);
-  const CUtensorMap map_b = plane_map(rb, 2 * (int64_t)n_mod * n, ldk);
+  const CUtensorMap map_a = plane_map(ra, 2 * (int64_t)n_mod * m, ldk, T2_BK, T2_M, CU_TENSOR_MAP_SWIZZLE_128B);
+  const CUtensorMap map_b = plane_map(rb, 2 * (int64_t)n_mod * n, ldk, T2_BK, T2_N, CU_TENSOR_MAP_SWIZZLE_128B);
   dim3 grid((unsigned)((m + T2_M - 1) / T2_M), (unsigned)((n + T2_N - 1) / T2_N), (unsigned)(n_mod * n_chunks));
   LAUNCH(ctx, k_i8_gemm_tc2, grid, T2_THREADS, T2_SMEM, map_a, map_b, m, n, ldk, n_mod, n_chunks, chunk_len, part, upper_only ? 1 : 0);
   const int64_t tot = 2 * (int64_t)n_mod * m * n;

@@ -437,9 +437,9 @@ struct BatchExec {
     for (Op* o : ops) v.push_back(get(o));
     return v;
   }
-  static unsigned gx_for(long long total) {
+  unsigned gx_for(long long total) const {
     long long g = (total + 255) / 256;
-    return (unsigned)std::max<long long>(1, std::min<long long>(g, 148 * 32));
+    return (unsigned)std::max<long long>(1, std::min<long long>(g, (long long)ctx->sm_count * 32));
   }
 
   void gram_batch(std::vector<GramItem>& v) {
@@ -947,7 +947,7 @@ struct Lobpcg {
   void gram(const std::vector<Mat>& A, const std::vector<Mat>& B, cplx* C, int64_t ldc, bool upper_only) {
     if (small) return small_gram(A, B, C, ldc, upper_only);
     if (!A.empty() && use_i8(A[0].rows)) {
-      // INT8 tensor cores (tcgen05.mma.kind::i8, TMA-fed; i8emu.cu / i8tc2.cu): every distinct block is converted to residue
+      // INT8 tensor cores (wgmma s8, TMA-fed; i8emu.cu / i8tc2.cu): every distinct block is converted to residue
       // planes once and enters all its block products
       bool ok = A.size() + B.size() <= N_PLANE_SLOTS;
       for (auto& a : A) ok = ok && a.cols >= 32;

@@ -131,7 +131,7 @@ void symmetrize_fourier(dftk_b200_grid* g, const cplx* in, cplx* out, int n_sym,
                         const double* tau_host);
 // i8emu.cu (experimental, option gemm_backend = 2)
 void zgemm_i8_cn(dftk_b200_ctx* ctx, int64_t m, int64_t n, int64_t k, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
-                 cplx* C, int64_t ldc, int tc_mode, const signed char* ra_cached = nullptr, const int* ea_cached = nullptr);
+                 cplx* C, int64_t ldc, bool tensor_cores, const signed char* ra_cached = nullptr, const int* ea_cached = nullptr);
 void i8tc2_products(dftk_b200_ctx* ctx, const signed char* ra, const signed char* rb, int64_t m, int64_t n, int64_t ldk,
                     int n_mod, short* part, int* res, bool upper_only);
 I8Operand i8_prepare(dftk_b200_ctx* ctx, const cplx* X, int64_t ld, int64_t cols, int64_t k, DevBuf<signed char>& store,
@@ -145,10 +145,6 @@ void i8tc2_products_nn(dftk_b200_ctx* ctx, int n_blocks, const signed char* cons
 void i8tc2_set_attributes();
 bool zgemm_i8_nn(dftk_b200_ctx* ctx, int64_t m, int64_t n, int64_t k, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
                  cplx* C, int64_t ldc, bool accumulate);
-// i8tc.cu (experimental, option gemm_backend = 3): tcgen05.mma.kind::i8 kernel of the integer products
-void i8tc_products(dftk_b200_ctx* ctx, const signed char* ra, const signed char* rb, int64_t m, int64_t n, int64_t ldk,
-                   int n_mod, short* part, int* res);
-void i8tc_set_attributes();
 // forces.cu
 void local_forces(dftk_b200_grid* g, const cplx* w, int n_atoms, const double* pos_host, double* out_host);
 void kb_nonlocal_force_rows(dftk_b200_kblock* kb, const cplx* psi, const double* occ_w_host, int64_t n_bands,

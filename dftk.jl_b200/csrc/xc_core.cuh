@@ -2,7 +2,7 @@
 // plumbing next to the hot path, SURVEY §8f rank 1; K16 of SURVEY §2.5).
 //
 // XC: the reference evaluates libxc through Libxc.jl (src/DispatchFunctional.jl:55-56,108-128; call site
-// src/terms/xc.jl:104-113).  libxc is third-party code that is not under /root/reference; the closed forms are
+// src/terms/xc.jl:104-113).  libxc is third-party code that is not under the DFTK.jl tree; the closed forms are
 // restated here (Dirac exchange, VWN5, PW92 / PW92-mod, PBE) with libxc's constants.  Energies per volume `e`
 // and the derivatives vrho / vsigma come from ONE expression evaluated on forward-mode dual numbers, so they are
 // mutually consistent by construction.

@@ -30,7 +30,7 @@ class Context:
     def __init__(self, device=0, nccl_id=None, rank=0, nranks=1):
         self.L = _lib.lib()
         if not torch.cuda.is_available():
-            raise RuntimeError("dftk_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("dftk_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         torch.cuda.set_device(device)
         torch.zeros(1, device=f"cuda:{device}")  # make sure the primary context exists
         h = c_vp()

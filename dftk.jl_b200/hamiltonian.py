@@ -26,7 +26,7 @@ class DftHamiltonianBlock:
         nonloc = [o for o in ops if isinstance(o, NonlocalOperator)]
         if len(fourier) > 1 or len(nonloc) > 1 or len(fourier) + len(real) + len(nonloc) != len(ops):
             raise NotImplementedError("only DFT Hamiltonians (one Fourier multiplication, local potentials, "
-                                      "at most one nonlocal operator) are supported by the B200 back end")
+                                      "at most one nonlocal operator) are supported by this GPU back end")
         self.fourier_op = fourier[0] if fourier else None
         self.nonlocal_op = nonloc[0] if nonloc else None
         # optimize_operators (operators.jl:213-222): sum all real-space multiplications

@@ -1,5 +1,5 @@
 /*
- * libdftk_b200 -- C ABI of the B200-native plane-wave Kohn-Sham hot path.
+ * libdftk_b200 -- C ABI of the H100-native (sm_90a) plane-wave Kohn-Sham hot path.
  *
  * Drop-in boundary for the seam where DFTK.jl's ext/DFTKCUDAExt.jl + src/architecture.jl plug in
  * today (reference paths relative to the DFTK.jl tree).  Each entry point names the reference
@@ -59,16 +59,15 @@ int64_t dftk_b200_sync_count(dftk_b200_ctx* ctx, int reset);
  * (8 rows·m·n, half of it for the upper-triangle-only diagonal blocks), update-type products, the X R^-1 updates of ortho! and the
  * two projector products of every H apply -- the "sum actually executed" of SURVEY §8d.  Batched small-block solves are not counted. */
 double dftk_b200_lobpcg_flops(dftk_b200_ctx* ctx, int reset);
-/* tuning knobs: "gemm_backend" (4 = default: the Gram-type and update-type products of contractions with at least
- * "i8_min_rows" (32768) rows run on the INT8 tensor cores -- tcgen05.mma.kind::i8 fed by TMA, FP64-equivalent results through
- * INT8 residues + CRT -- and everything smaller on the own FP64 DMMA kernels; 0 = DMMA kernels only; 1 = cuBLAS, for A/B
- * comparison and peak calibration only; 2 / 3 = checkers of the INT8 scheme: integer products on CUDA cores / cp.async-fed
- * tensor-core kernel), "gemm_stages" (cp.async ring depth 2|3 of the DMMA kernels), "band_chunk" (bands per batched-FFT
+/* tuning knobs: "gemm_backend" (0 = default: own FP64 DMMA kernels; 4 = the Gram-type and update-type products of
+ * contractions with at least "i8_min_rows" (32768) rows on the INT8 tensor cores -- wgmma s8 fed by TMA, FP64-equivalent results
+ * through INT8 residues + CRT -- and everything smaller on the DMMA kernels; 1 = cuBLAS, for A/B comparison and peak calibration
+ * only; 2 = checker of the INT8 scheme: integer products on CUDA cores), "gemm_stages" (cp.async ring depth 2|3 of the DMMA kernels), "band_chunk" (bands per batched-FFT
  * launch, 0 = auto), "fft_engine" (0 = register two-pass engine where a factor pair exists, 1 = generic Stockham; applies to
  * grids created afterwards), "small_dense" (1 = batched small-matrix path for LOBPCG solves with <= 32 bands, 0 = the GEMM +
  * cuSOLVER sequence of the large path), "z_pipeline" (1 = persistent cp.async-pipelined fused z stage; default 0),
  * "batch_pipeline" (1 = batched solves of >= 8 k-blocks run as two groups on two streams so that one group's host work hides
- * behind the other's kernels; 0 = one group, one stream synchronisation per round; default 0: measured no faster),
+ * behind the other's kernels; 0 = one group, one stream synchronisation per round; default 0),
  * "force_svd_fallback" (test hook) */
 int dftk_b200_set_option(dftk_b200_ctx* ctx, const char* name, int64_t value);
 

@@ -9,7 +9,7 @@ fails loudly if its CUDA library is missing.
 Why a restatement: the reference is pure Julia and `julia` is not installed in the build
 or measurement containers (no network), so the reference itself cannot be imported or
 compiled.  Every function cites the reference file:line it follows (paths relative to
-/root/reference).  Parity pins (all checked in tests/test_oracle_golden.py):
+the DFTK.jl tree).  Parity pins (all checked in tests/test_oracle_golden.py):
   * test/PspHgh.jl:41-84           HGH local / projector Fourier values
   * test/energy_nuclear.jl:31,48   Ewald, psp correction (ABINIT numbers)
   * test/compute_fft_size.jl:6-12  FFT grid sizes
@@ -17,7 +17,7 @@ compiled.  Every function cites the reference file:line it follows (paths relati
   * test/lobpcg.jl:13-22,63-103    free-electron, kinetic+local(+nonlocal) eigenvalues
   * test/energies_guess_density.jl:8-36   every energy term of LDA silicon to 5e-8
   * test/silicon_lda.jl:10-20      full SCF vs ABINIT eigenvalues / total energy
-Third-party arithmetic restated from published formulas (not in /root/reference):
+Third-party arithmetic restated from published formulas (not in the DFTK.jl tree):
 libxc (lda_x, lda_c_vwn, lda_c_pw, gga_x_pbe, gga_c_pbe), pinned through the energy
 values above; spglib is avoided (symmetries found by brute force over lattice isometries).
 """

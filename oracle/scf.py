@@ -220,7 +220,7 @@ def kerker_mix(basis, dF, kTF=0.8):
 def gmres(apply, b, rtol=0.01, atol=1e-12, krylovdim=30, maxiter=100):
     """Restarted GMRES from x0 = 0 (modified Gram-Schmidt Arnoldi, Givens rotations), the published algorithm behind the
     `KrylovKit.linsolve(f, b; rtol, ishermitian=false)` call of mixing.jl:283 (KrylovKit is a third-party dependency, compat
-    "0.8.3, 0.9, 0.10", not under /root/reference): stop when the residual estimate is below max(atol, rtol ||b||)."""
+    "0.8.3, 0.9, 0.10", not under the DFTK.jl tree): stop when the residual estimate is below max(atol, rtol ||b||)."""
     b = np.asarray(b, dtype=float)
     shape = b.shape
     b = b.reshape(-1)

@@ -1,7 +1,7 @@
 """Exchange-correlation functionals (oracle; test infrastructure only).
 
 The reference evaluates XC through Libxc.jl (src/DispatchFunctional.jl:55-56,108-128) -- third
-party arithmetic that is not under /root/reference (Libxc.jl compat "0.3.24", libxc C library
+party arithmetic that is not under the DFTK.jl tree (Libxc.jl compat "0.3.24", libxc C library
 unpinned).  Restated here from the published closed forms with libxc's constants:
   lda_x      Dirac/Slater exchange
   lda_c_vwn  Vosko-Wilk-Nusair 1980 (VWN5, RPA-free fit), libxc lda_c_vwn

@@ -1,4 +1,4 @@
-"""Development probe: the INT8-residue emulation of C = A^H B (gemm_backend 3: tcgen05.mma.kind::i8 integer products)
+"""Development probe: the INT8-residue emulation of C = A^H B (gemm_backend 4: wgmma s8 integer products)
 against the FP64 DMMA kernel (backend 0) and cuBLAS (backend 1) at the C3 nonlocal shape  P^H psi
 (K = 264 859, m = n_proj = 1250, n = 503 bands) and at the Gram shape (m = n = 1509)."""
 import sys, os, json
@@ -27,7 +27,7 @@ def timeit(fn, n=3, warm=1):
 
 
 SHAPES = (("nonlocal_PHpsi", 1250, 503),) if os.environ.get("ONLY_NONLOCAL") else (("nonlocal_PHpsi", 1250, 503), ("gram", 1509, 1509))
-BACKENDS = tuple(int(b) for b in os.environ.get("BACKENDS", "0,1,3").split(","))
+BACKENDS = tuple(int(b) for b in os.environ.get("BACKENDS", "0,1,4").split(","))
 for name, m, n in SHAPES:
     decay = torch.exp(-torch.linspace(0, 20, K, dtype=torch.float64, device=dev))
     A = torch.view_as_complex(torch.randn(m, K, 2, generator=g, device=dev, dtype=torch.float64)) * decay.sqrt() / np.sqrt(K)

@@ -1,4 +1,4 @@
-"""Development probe: section timing of one LOBPCG solve at the C3 shape (DFTK_B200_PROFILE=1)."""
+"""Development probe: section timing of one LOBPCG solve at the benchmark shape (DFTK_B200_PROFILE=1)."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 os.environ["DFTK_B200_PROFILE"] = "1"
@@ -8,7 +8,7 @@ sys.argv = ["bench.py"]
 import bench
 import dftk_b200 as dftk
 
-lat, pos = bench.supercell(int(os.environ.get("REP", 5)))
+lat, pos = bench.supercell(int(os.environ.get("REP", 4)))
 Si = dftk.ElementPsp("Si")
 model = dftk.model_DFT(lat, [Si] * len(pos), pos, functionals=dftk.LDA(), symmetries=False)
 basis = dftk.PlaneWaveBasis(model, Ecut=30.0, kgrid=dftk.ExplicitKpoints([[0, 0, 0]]))
@@ -30,7 +30,7 @@ for backend in [int(b) for b in os.environ.get("BACKENDS", "0").split(",")]:
     lams[backend] = res["λ"]
     print("gemm_backend", backend, "lobpcg", dt, "s", res["n_iter"], "iterations ->", dt / max(1, res["n_iter"]), "s/iteration", res["n_matvec"],
           res["converged"], "max resid", float(np.max(res["residual_norms"][:M - 3])), flush=True)
-ctx.set_option("gemm_backend", 4)
+ctx.set_option("gemm_backend", 0)
 if len(lams) > 1:
     ks = sorted(lams)
     print("max |eigenvalue difference| between backends", ks, ":", float(np.abs(lams[ks[0]] - lams[ks[-1]]).max()))

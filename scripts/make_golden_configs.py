@@ -23,18 +23,18 @@ def config(name):
     if name in ("C1", "C2"):
         lat = np.array([[0, A_SI, A_SI], [A_SI, 0, A_SI], [A_SI, A_SI, 0]])
         m = Model(lat, [Element("Si")] * 2, [np.ones(3) / 8, -np.ones(3) / 8], functionals=("lda_x", "lda_c_pw"))
-        return m, dict(Ecut=15, kgrid=(4, 4, 4)) if name == "C1" else dict(Ecut=30, kgrid=(8, 8, 8)), "simple", 1e-9
+        return m, dict(Ecut=15, kgrid=(4, 4, 4)) if name == "C1" else dict(Ecut=30, kgrid=(8, 8, 8)), "simple", 1e-10
     if name == "C4":
         a = 7.65339
         pos = [[0, 0, 0], [0, 0.5, 0.5], [0.5, 0, 0.5], [0.5, 0.5, 0]]
         m = Model(a * np.eye(3), [Element("Al", functional="pbe")] * 4, pos, functionals=("gga_x_pbe", "gga_c_pbe"),
                   temperature=0.01)
-        return m, dict(Ecut=40, kgrid=(12, 12, 12)), "kerker", 1e-8
+        return m, dict(Ecut=40, kgrid=(12, 12, 12)), "kerker", 1e-10
     if name == "C5":
         lat = 2.71176 * np.array([[-1, 1, 1], [1, -1, 1], [1, 1, -1]], dtype=float)
         m = Model(lat, [Element("Fe", functional="pbe")], [[0, 0, 0]], functionals=("gga_x_pbe", "gga_c_pbe"),
                   temperature=0.01, magnetic_moments=[4.0])
-        return m, dict(Ecut=45, kgrid=(8, 8, 8)), "kerker", 1e-8
+        return m, dict(Ecut=45, kgrid=(8, 8, 8)), "kerker", 1e-10
     raise KeyError(name)
 
 

@@ -32,6 +32,9 @@ if case == "slab":
     i8_rows = int(os.environ.get("I8_MIN_ROWS", "32768"))
     basis = dftk.PlaneWaveBasis(model, Ecut=Ecut, kgrid=(1, 1, 1), fft_size=(fft,) * 3, comm_slab=comm)
     assert basis.architecture.device.index == local and len(basis.kpoints) == 1
+    # I8_MIN_ROWS selects the INT8 tensor-core path (gemm_backend 4) for contractions of at least that many rows
+    i8_backend = 4 if "I8_MIN_ROWS" in os.environ else 0
+    basis.architecture.ctx.set_option("gemm_backend", i8_backend)
     basis.architecture.ctx.set_option("i8_min_rows", i8_rows)
     # eigensolver alone first: same start vectors, slab solve vs this rank's own single-GPU solve of the same block
     ham = dftk.energy_hamiltonian(basis, None, None, rho=dftk.guess_density(basis))[1]
@@ -52,6 +55,7 @@ if case == "slab":
     out = None
     if rank == 0:
         basis1 = dftk.PlaneWaveBasis(model, Ecut=Ecut, kgrid=(1, 1, 1), fft_size=(fft,) * 3, architecture=dftk.B200(local))
+        basis1.architecture.ctx.set_option("gemm_backend", i8_backend)
         basis1.architecture.ctx.set_option("i8_min_rows", i8_rows)
         ref = dftk.self_consistent_field(basis1, tol=1e-9)
         nocc = 4 * len(pos) // 2

@@ -1,6 +1,6 @@
 """Numerics study (CPU, NumPy): emulating the FP64 complex GEMMs of the nonlocal projector P'psi with INT8 products and
-INT32 accumulation -- the arithmetic `tcgen05.mma.kind::i8` provides on B200 -- so that the GEMM-shaped half of H psi can
-move from the FP64 DMMA pipe (~37 TFLOP/s) to the 5th-generation tensor cores.  Two error-free schemes:
+INT32 accumulation -- the arithmetic of the INT8 tensor-core MMAs (`wgmma` s8 -> s32 on sm_90a) -- so that the GEMM-shaped
+half of H psi can move from the FP64 DMMA pipe to the INT8 tensor cores.  Two error-free schemes:
 
   I.  slicing (Ozaki 2012 / ozIMMU): row-scaled operands are cut into s slices of `bits` bits; all slice pairs with
       i + j < s are multiplied exactly in integers: s(s+1)/2 int8 GEMMs.

@@ -20,7 +20,7 @@
 int main(void) {
   dftk_b200_ctx* ctx = NULL;
   if (dftk_b200_ctx_create(0, &ctx) != 0) {
-    fprintf(stderr, "no sm_100 device: %s\n", dftk_b200_last_error(NULL));
+    fprintf(stderr, "no sm_90 device: %s\n", dftk_b200_last_error(NULL));
     return 77;
   }
   const int n = 12;                       /* 12^3 cube, sphere = |G|^2 <= 16 in integer units */

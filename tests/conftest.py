@@ -13,5 +13,5 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100, sm_90a)")
     config.addinivalue_line("markers", "slow: longer CPU test")

@@ -59,13 +59,16 @@ def test_product_does_not_import_oracle():
                 assert "oracle/" not in src, f
 
 
-def test_sm100a_code_and_dmma_in_library(built):
+def test_sm90a_code_and_dmma_in_library(built):
     out = subprocess.run(["cuobjdump", "-lelf", built], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run(["cuobjdump", "-sass", "-fun", "_ZN4dftk10k_zgemm_cnILi2EEEvPK7double2lS3_lPS1_lllli", built],
                           capture_output=True, text=True).stdout
     assert "DMMA" in sass and "LDGSTS" in sass      # FP64 tensor-core MMA fed by cp.async staging
-    # register two-pass FFT stage for the 192-point axis of the headline workload is in the library
+    # INT8 residue products: warpgroup MMAs (wgmma s8) fed by TMA
+    sass = subprocess.run(["cuobjdump", "-sass", built], capture_output=True, text=True).stdout
+    assert "IGMMA" in sass and "UTMALDG" in sass
+    # register two-pass FFT stage for 192-point axes (the 192^3 grid of the 250-atom Si cell) is in the library
     elf = subprocess.run(["cuobjdump", "-elf", built], capture_output=True, text=True).stdout
     assert "kr_z_applyILi12ELi16E" in elf
 
@@ -87,7 +90,7 @@ def test_c_program_links_against_the_library(built, tmp_path):
     if torch.cuda.is_available():
         assert r.returncode == 0, r.stdout + r.stderr
     else:
-        assert r.returncode == 77 and "no sm_100 device" in r.stderr, (r.returncode, r.stderr)
+        assert r.returncode == 77 and "no sm_90 device" in r.stderr, (r.returncode, r.stderr)
 
 
 @pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""GPU parity tests of every kernel family against the CPU oracle (run on the B200 box: -m gpu).
+"""GPU parity tests of every kernel family against the CPU oracle (run on an H100: -m gpu).
 All calls go through the C ABI (ctypes)."""
 import os
 import numpy as np
@@ -76,7 +76,7 @@ def test_apply_h_terms(si, backend):
         check(kb.ctx.L.dftk_b200_apply_h(kb.h, _ptr(psi), _ptr(hout), psi.shape[0]), kb.ctx.h)
         np.testing.assert_allclose(hout, blk.matmul(psi.T).T, atol=1e-12 * scale)
     finally:
-        ctx().set_option("gemm_backend", 4)
+        ctx().set_option("gemm_backend", 0)
 
 
 @pytest.mark.parametrize("shape", [(1000, 7, 5), (4099, 70, 33), (129, 64, 32), (20000, 130, 1), (515, 3, 97)])
@@ -121,7 +121,7 @@ def test_band_energies_and_density(si):
     np.testing.assert_allclose(rho.cpu().numpy(), ref, atol=1e-12 * ref.max())
 
 
-@pytest.mark.parametrize("backend", [2, 3, 4])   # 2: integer products on CUDA cores, 3 / 4: tcgen05.mma.kind::i8 (cp.async-fed i8tc.cu / TMA-fed i8tc2.cu)
+@pytest.mark.parametrize("backend", [2, 4])   # 2: integer products on CUDA cores, 4: wgmma s8 on the tensor cores (TMA-fed, i8tc2.cu)
 @pytest.mark.parametrize("shape", [(3000, 7, 5), (70000, 20, 9), (140000, 150, 130)])
 def test_i8_emulated_gemm_matches_fp64(shape, backend):
     from gpu_common import ctx
@@ -140,11 +140,11 @@ def test_i8_emulated_gemm_matches_fp64(shape, backend):
         C = torch.zeros_like(ref)
         c.zgemm("C", A, B, C)
     finally:
-        c.set_option("gemm_backend", 4)
+        c.set_option("gemm_backend", 0)
         c.set_option("i8_min_rows", 32768)
     assert (C - ref).abs().max().item() < 1e-14 * ref.abs().max().item() * K ** 0.5
     if backend == 4:
-        # update type on the tensor cores (A as the MN-major UMMA operand, its column scales folded into S): X = A S (+ X0)
+        # update type on the tensor cores (A as the MN-major operand, its column scales folded into S): X = A S (+ X0)
         S = torch.view_as_complex(torch.randn(n, m, 2, generator=g, dtype=torch.float64)).to(c.device)
         X0 = torch.view_as_complex(torch.randn(n, K, 2, generator=g, dtype=torch.float64)).to(c.device)
         want = torch.zeros_like(X0)
@@ -158,7 +158,7 @@ def test_i8_emulated_gemm_matches_fp64(shape, backend):
             Xa = X0.clone()
             c.zgemm("N", A, S, Xa, -1.0, 1.0)
         finally:
-            c.set_option("gemm_backend", 4)
+            c.set_option("gemm_backend", 0)
             c.set_option("i8_min_rows", 32768)
         scale = (A.abs().max(dim=1).values[None, :] * S.abs()).sum(dim=1).max().item()      # sum_k |A[:,k]|max |S[k,j]|
         assert (X - want).abs().max().item() < 1e-14 * scale
@@ -176,7 +176,7 @@ def test_i8_emulated_gemm_matches_fp64(shape, backend):
             Xa = X0.clone()
             c.zgemm("N", A, S, Xa, 1.0, 1.0)
         finally:
-            c.set_option("gemm_backend", 4)
+            c.set_option("gemm_backend", 0)
         scale = (A.abs().max(dim=0).values[:, None] * S.abs().max()).max().item() * m
         assert (X - want).abs().max().item() < 1e-14 * scale
         assert (Xa - X0 - want).abs().max().item() < 1e-14 * scale
@@ -218,7 +218,7 @@ def test_lobpcg_matches_oracle(si, backend, small):
         assert res3["converged"]
         np.testing.assert_allclose(res3["λ"], ref["λ"][:6], atol=1e-7)
     finally:
-        ctx().set_option("gemm_backend", 4)
+        ctx().set_option("gemm_backend", 0)
         ctx().set_option("small_dense", 1)
 
 

@@ -302,7 +302,7 @@ def test_supercell_identity(rep, Ecut, fft):
 
 def test_supercell_identity_on_int8_tensor_cores():
     """The same identity (rep = 3: 54 atoms, 111 bands, 72^3 grid) with the Gram products of LOBPCG and the P'psi projection
-    on the INT8 tensor cores (gemm_backend 4: FP64 emulated by INT8 residues + CRT, tcgen05.mma.kind::i8 fed by TMA): the
+    on the INT8 tensor cores (gemm_backend 4: FP64 emulated by INT8 residues + CRT, wgmma s8 fed by TMA): the
     converged energy must still equal 27 x the primitive cell's to 1e-8 Ha per cell."""
     import dftk_b200 as dftk
     Si = dftk.ElementPsp("Si")
@@ -319,7 +319,7 @@ def test_supercell_identity_on_int8_tensor_cores():
     try:
         rs = dftk.self_consistent_field(bs, tol=1e-9)
     finally:
-        ctx.set_option("gemm_backend", 4)
+        ctx.set_option("gemm_backend", 0)
         ctx.set_option("i8_min_rows", 32768)
     assert rs["converged"] and ru["converged"]
     assert abs(rs["energies"].total - n * ru["energies"].total) < n * 1e-8

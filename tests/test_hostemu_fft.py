@@ -340,7 +340,7 @@ def test_emulated_small_heev_matches_numpy(emu, n):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# INT8-emulated FP64 GEMM (i8emu_core.cuh; groundwork for a tcgen05 kind::i8 path, not on the default path)
+# INT8-emulated FP64 GEMM (i8emu_core.cuh; the integer scheme behind gemm_backend 4)
 # ---------------------------------------------------------------------------------------------------------------
 I8_MODULI = [256, 255, 253, 251, 247, 241, 239, 233, 229, 227, 223, 217, 211, 199, 197, 193, 191, 181, 179, 173]
 
