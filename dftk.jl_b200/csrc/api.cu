@@ -239,7 +239,7 @@ int dftk_b200_set_option(dftk_b200_ctx* ctx, const char* name, int64_t value) {
     ctx->gemm_backend = (int)value;
   }
   else if (n == "band_chunk") ctx->band_chunk = (int)value;
-  else if (n == "gemm_stages") ctx->gemm_stages = (value == 3 ? 3 : 2);
+  else if (n == "gemm_stages") ctx->gemm_stages = (int)std::min<int64_t>(4, std::max<int64_t>(2, value));
   else if (n == "small_dense") ctx->small_dense = (int)value;
   else if (n == "i8_min_rows") ctx->i8_min_rows = value;
   else if (n == "z_pipeline") ctx->z_pipeline = (int)value;

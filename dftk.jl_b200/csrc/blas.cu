@@ -4,12 +4,15 @@
 //                src/eigen/lobpcg_hyper_impl.jl:90-113,216-221,277
 //   * zgemm_nn : C(K x n) = alpha * A(K x m) B(m x n) + beta * C              ("update" type:
 //                Hpsi += P (D P'psi), new_X = Y cX, X -= Y (BY'X), X = X invR) -- lobpcg_hyper_impl.jl:124-137
-// Both are real FP64 tensor-core GEMMs (mma.sync.m8n8k4.f64 = DMMA) on the interleaved complex
-// storage: with A~ the real (2K x m) view of A (rows re,im,re,im,...),
+// Both are real FP64 tensor-core GEMMs on the interleaved complex storage, built on mma.sync.m16n8k16.f64
+// (DMMA.16x8x16, 2048 MACs per warp instruction; Hopper's wgmma has no f64 form).  With A~ the real (2K x m) view of A
+// (rows re,im,re,im,...),
 //   Re(A^H B) = A~^T B~,   Im(A^H B) = A~^T (J B~),   (J b)[2k] = b[2k+1], (J b)[2k+1] = -b[2k]
 // and for the update C~ = A^ B~ with A^[:,2i] = A~[:,i], A^[:,2i+1] = J' A~[:,i].
-// The J-images are formed while loading MMA fragments from shared memory (index ^1 and a sign), so no
-// operand is ever materialised twice.  Tiles are staged with cp.async in a 3-stage ring.
+// The contraction index of an MMA may be permuted as long as both operands agree: the four k slots a lane holds
+// (t, t+4, t+8, t+12 with t = lane % 4) are mapped to the real indices 4t .. 4t+3, i.e. two whole complex numbers.
+// Fragments then load with LDS.128 and the J-images are formed in registers (a swap and a sign), so no operand is
+// ever materialised twice.  Tiles are staged with cp.async in a STAGES-deep ring (ctx->gemm_stages).
 #include "structs.cuh"
 
 namespace dftk {
@@ -24,118 +27,140 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
+// c += a b: A 16 x 16 (rows g, g+8 for a[even], a[odd]; k slot i/2), B 16 x 8 (k slot i, column g), C 16 x 8
+// (c[0..1]: row g, columns 2t, 2t+1; c[2..3]: row g+8), g = lane / 4, t = lane % 4
+__device__ __forceinline__ void dmma16(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+// sign flip with an integer XOR (ALU pipe, keeps the FP64 pipe free)
+__device__ __forceinline__ double neg(double x) {
+  return __hiloint2double(__double2hiint(x) ^ (int)0x80000000, __double2loint(x));
+}
+__device__ __forceinline__ double2 lds128(const double* p) { return *(const double2*)p; }
+// number of MMA tiles of `size` rows (at most `cap`) needed to cover `rem` remaining outputs
+__device__ __forceinline__ int mma_tiles(int64_t rem, int size, int cap) {
+  return rem <= 0 ? 0 : rem >= (int64_t)size * cap ? cap : (int)((rem + size - 1) / size);
 }
 
-#define GEMM_THREADS 128
-#define BKC 16              // complex k per stage (32 real)
-#define LDK (2 * BKC + 4)   // doubles per k-major smem row; LDK % 16 == 4 => conflict-free fragments
+#define GEMM_THREADS 256    // 8 warps, one CTA per SM (the accumulators and fragments take ~200 registers per thread)
+#define BKC 16              // complex k per stage (32 real: two k16 MMA steps)
+#define LDK (2 * BKC + 2)   // doubles per k-major smem row; LDK % 4 == 2 => the LDS.128 fragment loads of a quarter warp
+                            // (rows g, g+1; doubles 4t .. 4t+3) hit eight distinct 16-byte bank groups
 
 // ------------------------------------------------------------------------------------------------
-// Gram kernel.  CTA tile: 64 (i) x 32 (j) complex outputs; warp w owns i in [16w... no: rows 32*(w&1)..,
-// cols 16*(w>>1)..  => 4 warps = 2 x 2.  Partial sums over the K-slice [k_begin, k_end) are written to
-// ws[split][m x n]; reduce_partials applies alpha/beta.
+// Gram kernel.  CTA tile: 64 (i) x 96 (j) complex outputs; warp w owns i in 32 (w & 1) + [0, 32), j in 24 (w >> 1) +
+// [0, 24).  96 columns cover the 259 bands of the benchmark cell in 3 tiles (11 % padding).  Partial sums over the
+// K-slice [k_begin, k_end) are written to ws[split][m x n]; k_reduce_partials applies alpha/beta.
 // ------------------------------------------------------------------------------------------------
 #define GT_M 64
-#define GT_N 32
-template <int GEMM_STAGES>
-__global__ void __launch_bounds__(GEMM_THREADS)
+#define GT_N 96
+template <int STAGES>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_zgemm_cn(const cplx* __restrict__ A, int64_t lda, const cplx* __restrict__ B, int64_t ldb,
            cplx* __restrict__ ws, int64_t m, int64_t n, int64_t K, int64_t k_per_split, int upper_only) {
   // Hermitian results (X'X, X'AX): tiles strictly below the diagonal are never read by the callers
   if (upper_only && (int64_t)blockIdx.x * GT_M >= (int64_t)blockIdx.y * GT_N + GT_N) return;
   extern __shared__ __align__(16) double smem_d[];
-  double* As = smem_d;                                   // [STAGES][GT_M][LDK]
-  double* Bs = smem_d + GEMM_STAGES * GT_M * LDK;        // [STAGES][GT_N][LDK]
+  double* As = smem_d;                              // [STAGES][GT_M][LDK]
+  double* Bs = smem_d + STAGES * GT_M * LDK;        // [STAGES][GT_N][LDK]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t i0 = (int64_t)blockIdx.x * GT_M, j0 = (int64_t)blockIdx.y * GT_N;
   const int64_t kb = (int64_t)blockIdx.z * k_per_split;
   const int64_t ke = min(K, kb + k_per_split);
   const int nkt = (int)((ke - kb + BKC - 1) / BKC);
-  const int wi = (warp & 1) * 32, wj = (warp >> 1) * 16;
+  const int wi = (warp & 1) * 32, wj = (warp >> 1) * 24;
 
-  // Per-thread copy plan (fixed across k tiles): element e = tid + 128 i -> column tid/16 + 8 i, row tid%16.
+  // Per-thread copy plan (fixed across k tiles): element e = tid + 256 r -> column tid/16 + 16 r, k tid%16.
   const int lkk = tid & (BKC - 1), lcol = tid >> 4;
   const cplx* pA = A + kb + lkk + lda * (i0 + lcol);
   const cplx* pB = B + kb + lkk + ldb * (j0 + lcol);
   unsigned okA = 0, okB = 0;   // column-in-range masks
 #pragma unroll
-  for (int i = 0; i < GT_M / 8; ++i) okA |= (i0 + lcol + 8 * i < m) ? (1u << i) : 0u;
+  for (int r = 0; r < GT_M / 16; ++r) okA |= (i0 + lcol + 16 * r < m) ? (1u << r) : 0u;
 #pragma unroll
-  for (int i = 0; i < GT_N / 8; ++i) okB |= (j0 + lcol + 8 * i < n) ? (1u << i) : 0u;
+  for (int r = 0; r < GT_N / 16; ++r) okB |= (j0 + lcol + 16 * r < n) ? (1u << r) : 0u;
   auto load_tile = [&](int kt, int slot) {
     const int64_t koff = (int64_t)kt * BKC;
     const bool rowok = kb + koff + lkk < ke;
     double* da = As + ((size_t)slot * GT_M + lcol) * LDK + 2 * lkk;
     double* db = Bs + ((size_t)slot * GT_N + lcol) * LDK + 2 * lkk;
 #pragma unroll
-    for (int i = 0; i < GT_M / 8; ++i) {
-      bool ok = rowok && ((okA >> i) & 1u);
-      cp_async16(da + (size_t)8 * i * LDK, ok ? (pA + koff + (int64_t)8 * i * lda) : A, ok);
+    for (int r = 0; r < GT_M / 16; ++r) {
+      bool ok = rowok && ((okA >> r) & 1u);
+      cp_async16(da + (size_t)16 * r * LDK, ok ? (pA + koff + (int64_t)16 * r * lda) : A, ok);
     }
 #pragma unroll
-    for (int i = 0; i < GT_N / 8; ++i) {
-      bool ok = rowok && ((okB >> i) & 1u);
-      cp_async16(db + (size_t)8 * i * LDK, ok ? (pB + koff + (int64_t)8 * i * ldb) : B, ok);
+    for (int r = 0; r < GT_N / 16; ++r) {
+      bool ok = rowok && ((okB >> r) & 1u);
+      cp_async16(db + (size_t)16 * r * LDK, ok ? (pB + koff + (int64_t)16 * r * ldb) : B, ok);
     }
   };
 
-  double cr[4][2][2], ci[4][2][2];
+  double cr[2][3][4], ci[2][3][4];
 #pragma unroll
-  for (int a = 0; a < 4; ++a)
+  for (int a = 0; a < 2; ++a)
 #pragma unroll
-    for (int b = 0; b < 2; ++b) cr[a][b][0] = cr[a][b][1] = ci[a][b][0] = ci[a][b][1] = 0.0;
+    for (int b = 0; b < 3; ++b)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) cr[a][b][e] = ci[a][b][e] = 0.0;
 
-  for (int s = 0; s < GEMM_STAGES - 1; ++s) {
+  for (int s = 0; s < STAGES - 1; ++s) {
     if (s < nkt) load_tile(s, s);
     cp_async_commit();
   }
-  const int fr = lane >> 2, fk = lane & 3;
-  const int sgnmask = (lane & 1) ? (int)0x80000000 : 0;   // J-image sign, applied with an integer XOR (ALU pipe)
+  const int g = lane >> 2, t = lane & 3;
+  // MMA tiles of this warp that hold outputs (warp-uniform): narrow products skip the MMAs on padding
+  const int na = mma_tiles(m - i0 - wi, 16, 2), nb = mma_tiles(n - j0 - wj, 8, 3);
   for (int kt = 0; kt < nkt; ++kt) {
-    cp_async_wait<GEMM_STAGES - 2>();
+    cp_async_wait<STAGES - 2>();
     __syncthreads();
     {
-      int nxt = kt + GEMM_STAGES - 1;
-      if (nxt < nkt) load_tile(nxt, nxt % GEMM_STAGES);
+      int nxt = kt + STAGES - 1;
+      if (nxt < nkt) load_tile(nxt, nxt % STAGES);
       cp_async_commit();
     }
-    const double* as = As + (size_t)(kt % GEMM_STAGES) * GT_M * LDK;
-    const double* bs = Bs + (size_t)(kt % GEMM_STAGES) * GT_N * LDK;
+    const double* as = As + (size_t)(kt % STAGES) * GT_M * LDK + 4 * t;
+    const double* bs = Bs + (size_t)(kt % STAGES) * GT_N * LDK + 4 * t;
 #pragma unroll
-    for (int s4 = 0; s4 < 2 * BKC / 4; ++s4) {
-      double af[4], bf[2], bh[2];
+    for (int ks = 0; ks < BKC / 8; ++ks) {
+      double af[2][8];
 #pragma unroll
-      for (int a = 0; a < 4; ++a) af[a] = as[(wi + 8 * a + fr) * LDK + 4 * s4 + fk];
-#pragma unroll
-      for (int b = 0; b < 2; ++b) {
-        const double* row = bs + (wj + 8 * b + fr) * LDK + 4 * s4;
-        bf[b] = row[fk];
-        double t = row[fk ^ 1];
-        bh[b] = __hiloint2double(__double2hiint(t) ^ sgnmask, __double2loint(t));
+      for (int a = 0; a < 2; ++a) {
+        const double* p = as + (wi + 16 * a + g) * LDK + 16 * ks;
+        const double2 x0 = lds128(p), x1 = lds128(p + 2), y0 = lds128(p + 8 * LDK), y1 = lds128(p + 8 * LDK + 2);
+        af[a][0] = x0.x; af[a][1] = y0.x; af[a][2] = x0.y; af[a][3] = y0.y;
+        af[a][4] = x1.x; af[a][5] = y1.x; af[a][6] = x1.y; af[a][7] = y1.y;
       }
 #pragma unroll
-      for (int a = 0; a < 4; ++a)
+      for (int b = 0; b < 3; ++b) {
+        const double* p = bs + (wj + 8 * b + g) * LDK + 16 * ks;
+        const double2 v0 = lds128(p), v1 = lds128(p + 2);
+        const double bf[4] = {v0.x, v0.y, v1.x, v1.y};
+        const double bh[4] = {v0.y, neg(v0.x), v1.y, neg(v1.x)};   // J-image
 #pragma unroll
-        for (int b = 0; b < 2; ++b) {
-          dmma(cr[a][b][0], cr[a][b][1], af[a], bf[b]);
-          dmma(ci[a][b][0], ci[a][b][1], af[a], bh[b]);
+        for (int a = 0; a < 2; ++a) {
+          if (a < na && b < nb) {
+            dmma16(cr[a][b], af[a], bf);
+            dmma16(ci[a][b], af[a], bh);
+          }
         }
+      }
     }
   }
   cp_async_wait<0>();
   cplx* out = ws + (size_t)blockIdx.z * m * n;
 #pragma unroll
-  for (int a = 0; a < 4; ++a)
+  for (int a = 0; a < 2; ++a)
 #pragma unroll
-    for (int b = 0; b < 2; ++b)
+    for (int b = 0; b < 3; ++b)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        int64_t gi = i0 + wi + 8 * a + fr;
-        int64_t gj = j0 + wj + 8 * b + 2 * fk + e;
+      for (int e = 0; e < 4; ++e) {
+        int64_t gi = i0 + wi + 16 * a + g + 8 * (e >> 1);
+        int64_t gj = j0 + wj + 8 * b + 2 * t + (e & 1);
         if (gi < m && gj < n) out[gi + m * gj] = make_double2(cr[a][b][e], ci[a][b][e]);
       }
 }
@@ -157,28 +182,31 @@ __global__ void k_reduce_partials(const cplx* __restrict__ ws, int nsplit, int64
 }
 
 // ------------------------------------------------------------------------------------------------
-// Update kernel.  CTA tile: 64 complex rows (128 real) x 32 columns; warp w owns real rows 32w..32w+31.
+// Update kernel.  CTA tile: 64 complex rows x 96 columns; warp w owns rows 32 (w & 1) + [0, 32), columns 24 (w >> 1) +
+// [0, 24).  An MMA covers 8 complex rows: its rows g and g+8 are the real and imaginary parts of complex row g, so a
+// lane holds whole complex outputs and the epilogue needs no shuffles.
 // ------------------------------------------------------------------------------------------------
 #define UT_M 64                 // complex rows
-#define UT_N 32
-#define LDA_U (2 * UT_M + 4)    // doubles per inner-index row of the A tile (132 % 16 == 4)
-template <int GEMM_STAGES>
-__global__ void __launch_bounds__(GEMM_THREADS)
+#define UT_N 96
+#define LDA_U (2 * UT_M + 2)    // doubles per inner-index row of the A tile; LDA_U % 8 == 2 => conflict-free LDS.128
+template <int STAGES>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_zgemm_nn(const cplx* __restrict__ A, int64_t lda, const cplx* __restrict__ B, int64_t ldb,
            cplx* __restrict__ C, int64_t ldc, int64_t Krows, int64_t n, int64_t m, cplx alpha, cplx beta,
            int b_upper) {
   extern __shared__ __align__(16) double smem_d[];
-  double* As = smem_d;                                   // [STAGES][BKC][LDA_U]
-  double* Bs = smem_d + GEMM_STAGES * BKC * LDA_U;       // [STAGES][UT_N][LDK]
+  double* As = smem_d;                              // [STAGES][BKC][LDA_U]
+  double* Bs = smem_d + STAGES * BKC * LDA_U;       // [STAGES][UT_N][LDK]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // blockIdx.x = column tile (fastest): CTAs sharing one A row panel run together and hit it in L2
   const int64_t r0 = (int64_t)blockIdx.y * UT_M, j0 = (int64_t)blockIdx.x * UT_N;
   // B upper triangular (X * inv(R), rmul! with an UpperTriangular): rows i > j of column j are zero
   const int64_t m_eff = b_upper ? min(m, j0 + UT_N) : m;
   const int nkt = (int)((m_eff + BKC - 1) / BKC);
+  const int wr = (warp & 1) * 32, wj = (warp >> 1) * 24;
 
-  // Per-thread copy plan: A tile element e = tid + 128 i -> inner index e/64 = tid/64 + 2 i, row e%64 = tid%64;
-  //                       B tile element e = tid + 128 i -> column tid/16 + 8 i, inner index tid%16.
+  // Per-thread copy plan: A tile element e = tid + 256 r -> inner index e/64 = tid/64 + 4 r, row e%64 = tid%64;
+  //                       B tile element e = tid + 256 r -> column tid/16 + 16 r, inner index tid%16.
   const int arow = tid & (UT_M - 1), aii = tid >> 6;
   const int bii = tid & (BKC - 1), bcol = tid >> 4;
   const bool arow_ok = r0 + arow < Krows;
@@ -186,63 +214,69 @@ k_zgemm_nn(const cplx* __restrict__ A, int64_t lda, const cplx* __restrict__ B, 
   const cplx* pB = B + bii + ldb * (j0 + bcol);
   unsigned okB = 0;
 #pragma unroll
-  for (int i = 0; i < UT_N / 8; ++i) okB |= (j0 + bcol + 8 * i < n) ? (1u << i) : 0u;
+  for (int r = 0; r < UT_N / 16; ++r) okB |= (j0 + bcol + 16 * r < n) ? (1u << r) : 0u;
   auto load_tile = [&](int kt, int slot) {
     const int64_t i0 = (int64_t)kt * BKC;
     double* da = As + ((size_t)slot * BKC + aii) * LDA_U + 2 * arow;
     double* db = Bs + ((size_t)slot * UT_N + bcol) * LDK + 2 * bii;
 #pragma unroll
-    for (int i = 0; i < BKC / 2; ++i) {
-      bool ok = arow_ok && (i0 + aii + 2 * i < m_eff);
-      cp_async16(da + (size_t)2 * i * LDA_U, ok ? (pA + (i0 + 2 * i) * lda) : A, ok);
+    for (int r = 0; r < BKC / 4; ++r) {
+      bool ok = arow_ok && (i0 + aii + 4 * r < m_eff);
+      cp_async16(da + (size_t)4 * r * LDA_U, ok ? (pA + (i0 + 4 * r) * lda) : A, ok);
     }
     const bool iiok = i0 + bii < m_eff;
 #pragma unroll
-    for (int i = 0; i < UT_N / 8; ++i) {
-      bool ok = iiok && ((okB >> i) & 1u);
-      cp_async16(db + (size_t)8 * i * LDK, ok ? (pB + i0 + (int64_t)8 * i * ldb) : B, ok);
+    for (int r = 0; r < UT_N / 16; ++r) {
+      bool ok = iiok && ((okB >> r) & 1u);
+      cp_async16(db + (size_t)16 * r * LDK, ok ? (pB + i0 + (int64_t)16 * r * ldb) : B, ok);
     }
   };
 
-  double acc[4][4][2];
+  double acc[4][3][4];
 #pragma unroll
   for (int a = 0; a < 4; ++a)
 #pragma unroll
-    for (int b = 0; b < 4; ++b) acc[a][b][0] = acc[a][b][1] = 0.0;
+    for (int b = 0; b < 3; ++b)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[a][b][e] = 0.0;
 
-  for (int s = 0; s < GEMM_STAGES - 1; ++s) {
+  for (int s = 0; s < STAGES - 1; ++s) {
     if (s < nkt) load_tile(s, s);
     cp_async_commit();
   }
-  const int fr = lane >> 2, fk = lane & 3;
-  const int wr = warp * 32;
+  const int g = lane >> 2, t = lane & 3;
+  // MMA tiles of this warp that hold outputs (warp-uniform): narrow products skip the MMAs on padding
+  const int na = mma_tiles(Krows - r0 - wr, 8, 4), nb = mma_tiles(n - j0 - wj, 8, 3);
   for (int kt = 0; kt < nkt; ++kt) {
-    cp_async_wait<GEMM_STAGES - 2>();
+    cp_async_wait<STAGES - 2>();
     __syncthreads();
     {
-      int nxt = kt + GEMM_STAGES - 1;
-      if (nxt < nkt) load_tile(nxt, nxt % GEMM_STAGES);
+      int nxt = kt + STAGES - 1;
+      if (nxt < nkt) load_tile(nxt, nxt % STAGES);
       cp_async_commit();
     }
-    const double* as = As + (size_t)(kt % GEMM_STAGES) * BKC * LDA_U;
-    const double* bs = Bs + (size_t)(kt % GEMM_STAGES) * UT_N * LDK;
+    const double* as = As + (size_t)(kt % STAGES) * BKC * LDA_U + 2 * t * LDA_U + 2 * (wr + g);
+    const double* bs = Bs + (size_t)(kt % STAGES) * UT_N * LDK + 4 * t;
 #pragma unroll
-    for (int s4 = 0; s4 < 2 * BKC / 4; ++s4) {
-      double af[4], bf[4];
-      const int ii = 2 * s4 + (fk >> 1);
+    for (int ks = 0; ks < BKC / 8; ++ks) {
+      // k slots 4t .. 4t+3 = (inner 2t, re), (2t, im), (2t+1, re), (2t+1, im); rows g / g+8 = Re / Im of the output row:
+      //   Re row: Ar Br - Ai Bi,   Im row: Ai Br + Ar Bi
+      double bf[3][4];
 #pragma unroll
-      for (int a = 0; a < 4; ++a) {
-        int R = wr + 8 * a + fr;  // real row inside the tile
-        // A^[R][2i] = A~[R][i];  A^[R][2i+1] = (R odd) ? A~[R-1][i] : -A~[R+1][i]
-        double v = as[ii * LDA_U + ((fk & 1) ? (R ^ 1) : R)];
-        af[a] = ((fk & 1) && !(R & 1)) ? __hiloint2double(__double2hiint(v) ^ (int)0x80000000, __double2loint(v)) : v;
+      for (int b = 0; b < 3; ++b) {
+        const double* p = bs + (wj + 8 * b + g) * LDK + 16 * ks;
+        const double2 v0 = lds128(p), v1 = lds128(p + 2);
+        bf[b][0] = v0.x; bf[b][1] = v0.y; bf[b][2] = v1.x; bf[b][3] = v1.y;
       }
 #pragma unroll
-      for (int b = 0; b < 4; ++b) bf[b] = bs[(8 * b + fr) * LDK + 4 * s4 + fk];
+      for (int a = 0; a < 4; ++a) {
+        const double* p = as + 8 * ks * LDA_U + 16 * a;
+        const double2 z0 = lds128(p), z1 = lds128(p + LDA_U);
+        const double af[8] = {z0.x, z0.y, neg(z0.y), z0.x, z1.x, z1.y, neg(z1.y), z1.x};
 #pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = 0; b < 4; ++b) dmma(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+        for (int b = 0; b < 3; ++b)
+          if (a < na && b < nb) dmma16(acc[a][b], af, bf[b]);
+      }
     }
   }
   cp_async_wait<0>();
@@ -250,24 +284,15 @@ k_zgemm_nn(const cplx* __restrict__ A, int64_t lda, const cplx* __restrict__ B, 
 #pragma unroll
   for (int a = 0; a < 4; ++a)
 #pragma unroll
-    for (int b = 0; b < 4; ++b)
+    for (int b = 0; b < 3; ++b)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        int R = wr + 8 * a + fr;
-        double v = acc[a][b][e];
-        double partner = __shfl_xor_sync(0xffffffffu, v, 4);  // other component of the same complex entry
-        int64_t grow = r0 + (R >> 1);
-        int64_t gj = j0 + 8 * b + 2 * fk + e;
-        double o;
-        if (R & 1) o = alpha.x * v + alpha.y * partner;   // imaginary part: ar*im + ai*re
-        else o = alpha.x * v - alpha.y * partner;         // real part:      ar*re - ai*im
+        const int64_t grow = r0 + wr + 8 * a + g;
+        const int64_t gj = j0 + wj + 8 * b + 2 * t + e;
         if (grow < Krows && gj < n) {
-          double* cp = (double*)(C + grow + ldc * gj);
-          if (has_beta) {
-            double2 c = *(const double2*)cp;
-            o += (R & 1) ? (beta.x * c.y + beta.y * c.x) : (beta.x * c.x - beta.y * c.y);
-          }
-          cp[R & 1] = o;
+          cplx o = cmul(alpha, make_double2(acc[a][b][e], acc[a][b][2 + e]));
+          if (has_beta) o = cadd(o, cmul(beta, C[grow + ldc * gj]));
+          C[grow + ldc * gj] = o;
         }
       }
 }
@@ -351,6 +376,8 @@ void blas_set_attributes() {
   CUDA_CHECK(cudaFuncSetAttribute(k_zgemm_nn<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_nn(2)));
   CUDA_CHECK(cudaFuncSetAttribute(k_zgemm_cn<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cn(3)));
   CUDA_CHECK(cudaFuncSetAttribute(k_zgemm_nn<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_nn(3)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_zgemm_cn<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cn(4)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_zgemm_nn<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_nn(4)));
 }
 
 void columnwise_dots(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
@@ -408,18 +435,22 @@ void zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_t k, cplx
            alpha, beta, C, ldc);
     return;
   }
+  const int st = ctx->gemm_stages;
   if (transA == 2) {
-    int64_t tiles = ((m + GT_M - 1) / GT_M) * ((n + GT_N - 1) / GT_N);
-    // split K so that the CTA count fills whole waves (3 resident CTAs per SM) at least twice over
-    const int64_t slots = (ctx->gemm_stages == 3 ? 2 : 4) * (int64_t)ctx->sm_count;   // resident CTAs
-    int64_t max_split = std::min<int64_t>(64, (k + 8 * BKC - 1) / (8 * BKC));
+    // tiles that do work (Hermitian Grams skip the tiles strictly below the diagonal)
+    const int64_t mt = (m + GT_M - 1) / GT_M, nt = (n + GT_N - 1) / GT_N;
+    const bool upper = upper_only && m == n;
+    int64_t tiles = 0;
+    for (int64_t bj = 0; bj < nt; ++bj) tiles += upper ? std::min(mt, ((bj + 1) * GT_N + GT_M - 1) / GT_M) : mt;
+    // one CTA per SM is resident: split K so that the CTA count fills whole waves of sm_count, keeping >= 8 stages
+    // per split; the mild per-split penalty stands for the pipeline fill and the reduce pass
+    const int64_t slots = ctx->sm_count;
+    const int64_t max_split = std::min<int64_t>(64, (k + 8 * BKC - 1) / (8 * BKC));
     int64_t nsplit = 1;
     double best = -1.0;
     for (int64_t sp = 1; sp <= max_split; ++sp) {
-      int64_t total = tiles * sp;
-      double eff = (double)total / (double)(((total + slots - 1) / slots) * slots);
-      if (total < 2 * slots) eff *= 0.5 + 0.25 * (double)total / (double)slots;   // prefer >= 2 waves
-      eff -= 0.002 * sp;                                                          // mild penalty: reduce pass
+      const int64_t total = tiles * sp;
+      const double eff = (double)total / (double)(((total + slots - 1) / slots) * slots) - 0.002 * sp;
       if (eff > best) {
         best = eff;
         nsplit = sp;
@@ -429,24 +460,20 @@ void zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_t k, cplx
     kps = ((kps + BKC - 1) / BKC) * BKC;
     nsplit = (k + kps - 1) / kps;
     cplx* ws = (cplx*)ctx->gemm_ws.ensure((size_t)nsplit * m * n * sizeof(cplx));
-    dim3 grid((unsigned)((m + GT_M - 1) / GT_M), (unsigned)((n + GT_N - 1) / GT_N), (unsigned)nsplit);
-    if (ctx->gemm_stages == 3)
-      LAUNCH(ctx, k_zgemm_cn<3>, grid, GEMM_THREADS, smem_cn(3), A, lda, B, ldb, ws, m, n, k, kps,
-             (upper_only && m == n) ? 1 : 0);
-    else
-      LAUNCH(ctx, k_zgemm_cn<2>, grid, GEMM_THREADS, smem_cn(2), A, lda, B, ldb, ws, m, n, k, kps,
-             (upper_only && m == n) ? 1 : 0);
+    dim3 grid((unsigned)mt, (unsigned)nt, (unsigned)nsplit);
+    const int uo = upper ? 1 : 0;
+    if (st == 2) LAUNCH(ctx, k_zgemm_cn<2>, grid, GEMM_THREADS, smem_cn(2), A, lda, B, ldb, ws, m, n, k, kps, uo);
+    else if (st == 3) LAUNCH(ctx, k_zgemm_cn<3>, grid, GEMM_THREADS, smem_cn(3), A, lda, B, ldb, ws, m, n, k, kps, uo);
+    else LAUNCH(ctx, k_zgemm_cn<4>, grid, GEMM_THREADS, smem_cn(4), A, lda, B, ldb, ws, m, n, k, kps, uo);
     LAUNCH(ctx, k_reduce_partials, (unsigned)((m * n + 255) / 256), 256, 0, (const cplx*)ws, (int)nsplit, m,
            n, alpha, beta, C, ldc);
   } else {
     REQUIRE((m + UT_M - 1) / UT_M <= 65535, "zgemm: more than 4.19M rows are not supported by the update kernel grid");
     dim3 grid((unsigned)((n + UT_N - 1) / UT_N), (unsigned)((m + UT_M - 1) / UT_M));
-    if (ctx->gemm_stages == 3)
-      LAUNCH(ctx, k_zgemm_nn<3>, grid, GEMM_THREADS, smem_nn(3), A, lda, B, ldb, C, ldc, m, n, k, alpha, beta,
-             (upper_only && k == n) ? 1 : 0);
-    else
-      LAUNCH(ctx, k_zgemm_nn<2>, grid, GEMM_THREADS, smem_nn(2), A, lda, B, ldb, C, ldc, m, n, k, alpha, beta,
-             (upper_only && k == n) ? 1 : 0);
+    const int bu = (upper_only && k == n) ? 1 : 0;
+    if (st == 2) LAUNCH(ctx, k_zgemm_nn<2>, grid, GEMM_THREADS, smem_nn(2), A, lda, B, ldb, C, ldc, m, n, k, alpha, beta, bu);
+    else if (st == 3) LAUNCH(ctx, k_zgemm_nn<3>, grid, GEMM_THREADS, smem_nn(3), A, lda, B, ldb, C, ldc, m, n, k, alpha, beta, bu);
+    else LAUNCH(ctx, k_zgemm_nn<4>, grid, GEMM_THREADS, smem_nn(4), A, lda, B, ldb, C, ldc, m, n, k, alpha, beta, bu);
   }
 }
 

@@ -93,11 +93,12 @@ struct dftk_b200_ctx {
   int gemm_backend = 0;   // 0 (default) = own FP64 DMMA kernels; 4 = INT8 tensor cores (wgmma s8, TMA-fed; i8emu.cu / i8tc2.cu) for
                           // contractions of at least i8_min_rows rows, DMMA otherwise; 1 = cuBLAS (A/B comparison only); 2 = checker of
                           // the INT8 scheme (integer products on CUDA cores).  DMMA is the default because it is the faster of the two on
-                          // an H100 SXM (400 W): LOBPCG iteration of the 128-atom Si cell (259 bands) 0.18 s vs 0.27 s, nonlocal products
-                          // 19.2 ms vs 22.3 ms, equal eigenvalues to 1e-15
+                          // an H100 SXM (700 W): LOBPCG iteration of the 128-atom Si cell (259 bands) 0.12 s vs 0.21 s, nonlocal products
+                          // 9.8 ms vs 16.3 ms, equal eigenvalues to 2e-15
   int band_chunk = 0;     // 0 = auto
   int fft_engine = 0;     // 0 = register two-pass engine where a factor pair exists, 1 = generic Stockham (applies to grids created afterwards)
-  int gemm_stages = 2;    // cp.async ring depth of the DMMA GEMMs (2 -> 4 CTAs/SM, 3 -> 2 CTAs/SM)
+  int gemm_stages = 4;    // cp.async ring depth (2..4) of the DMMA GEMMs; one 8-warp CTA per SM at every depth (2, 3 and 4 time
+                          // within noise of each other on an H100; scripts/gemm_probe.py compares them)
   int64_t i8_min_rows = 32768;   // gemm_backend 4: shortest contraction length that goes to the INT8 tensor-core path
   int z_pipeline = 0;     // fused z stage of the H apply: 0 = one tile per CTA (default), 1 = persistent cp.async-pipelined kernel
   int force_svd_fallback = 0;   // test hook: the next N ortho! calls behave as if safe_cholesky had given up

@@ -62,7 +62,7 @@ double dftk_b200_lobpcg_flops(dftk_b200_ctx* ctx, int reset);
 /* tuning knobs: "gemm_backend" (0 = default: own FP64 DMMA kernels; 4 = the Gram-type and update-type products of
  * contractions with at least "i8_min_rows" (32768) rows on the INT8 tensor cores -- wgmma s8 fed by TMA, FP64-equivalent results
  * through INT8 residues + CRT -- and everything smaller on the DMMA kernels; 1 = cuBLAS, for A/B comparison and peak calibration
- * only; 2 = checker of the INT8 scheme: integer products on CUDA cores), "gemm_stages" (cp.async ring depth 2|3 of the DMMA kernels), "band_chunk" (bands per batched-FFT
+ * only; 2 = checker of the INT8 scheme: integer products on CUDA cores), "gemm_stages" (cp.async ring depth 2|3|4 of the DMMA kernels, default 4), "band_chunk" (bands per batched-FFT
  * launch, 0 = auto), "fft_engine" (0 = register two-pass engine where a factor pair exists, 1 = generic Stockham; applies to
  * grids created afterwards), "small_dense" (1 = batched small-matrix path for LOBPCG solves with <= 32 bands, 0 = the GEMM +
  * cuSOLVER sequence of the large path), "z_pipeline" (1 = persistent cp.async-pipelined fused z stage; default 0),
