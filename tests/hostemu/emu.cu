@@ -105,10 +105,11 @@ int emu_fft_cube(int nx, int ny, int nz, double* data, int sign, int batch) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Register two-pass engine (fft_reg.cuh) emulation: a few factor pairs are instantiated on the host.
+// Register two-pass engine (fft_reg.cuh) emulation: every factor pair of the device engine is instantiated on the host,
+// so a pair added to DFTK_REG_PAIRS is emulated (and tested) without further edits.
 // ------------------------------------------------------------------------------------------------
 #include "../../dftk.jl_b200/csrc/fft_reg.cuh"
-#define EMU_PAIRS(X) X(3, 5) X(3, 6) X(4, 6) X(3, 9) X(4, 4) X(4, 5)
+#define EMU_PAIRS(X) DFTK_REG_PAIRS(X)
 static bool emu_pair(int n, int* A, int* B) {
   *A = 0;
 #define PX(a, b) if (n == (a) * (b) && *A == 0) { *A = a; *B = b; }

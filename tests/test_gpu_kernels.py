@@ -344,25 +344,28 @@ def test_fft_engines_agree_with_oracle(fft_size, Ecut):
             ctx().set_option("fft_engine", 0)
 
 
-def test_full_size_properties_192():
-    """BASELINE full-size grid (192^3, the C3 cell): size-independent properties instead of an oracle run --
-    round trip, linearity, Hermiticity <phi|H psi> = <H phi|psi>, Parseval, density normalisation."""
+def _full_size_checks(rep, n, n_pw):
+    """Si rep x rep x rep supercell, Gamma, Ecut 30 Ha on an n^3 grid: size-independent properties instead of an oracle
+    run -- round trip, linearity, Hermiticity <phi|H psi> = <H phi|psi>, Parseval, density normalisation -- and
+    apply_terms(psi, 3) and sphere_to_real of three bands against numpy.fft (which test_fft_reference.py ties to the
+    direct DFT)."""
     import dftk_b200
     from gpu_common import ctx
     c = ctx()
     dev = c.device
     A = 10.26 / 2
-    lat = 5 * np.array([[0, A, A], [A, 0, A], [A, A, 0]])
+    lat = rep * np.array([[0, A, A], [A, 0, A], [A, A, 0]])
     recip = 2 * np.pi * np.linalg.inv(lat.T)
-    n = 192
-    g1 = torch.as_tensor(np.array(list(range(0, 96)) + list(range(-96, 0))), device=dev, dtype=torch.float64)
+    g1 = torch.as_tensor(np.array(list(range(0, (n + 1) // 2)) + list(range(-(n // 2), 0))), device=dev, dtype=torch.float64)
     Z, Y, X = torch.meshgrid(g1, g1, g1, indexing="ij")
     G = torch.stack([X.reshape(-1), Y.reshape(-1), Z.reshape(-1)], 1)
     p = G @ torch.as_tensor(recip.T, device=dev)
     kin_all = (p * p).sum(1) / 2
+    del G, p, X, Y, Z
     mapping = torch.nonzero(kin_all <= 30.0).reshape(-1)
-    assert mapping.numel() == 264859                               # SURVEY §8 table, config C3
+    assert mapping.numel() == n_pw
     kin = kin_all[mapping].contiguous()
+    del kin_all
     vol = abs(np.linalg.det(lat))
     grid = dftk_b200.FFTGrid(c, (n, n, n), vol)
     kb = dftk_b200.KBlock(grid, mapping.cpu().numpy(), kin=kin)
@@ -386,6 +389,31 @@ def test_full_size_properties_192():
     kb.density_accumulate(psi, np.full(6, 2.0), rho)
     assert abs(rho.sum().item() * (vol / n ** 3) - 12.0) < 1e-10
     assert rho.min().item() >= 0.0
+    del rho, H
+    # three bands against numpy.fft
+    mp, Vn, kn = mapping.cpu().numpy(), V.cpu().numpy().reshape(n, n, n), kin.cpu().numpy()
+    ps = psi[:3].contiguous()
+    hp = kb.apply_terms(ps, 3).cpu().numpy()
+    cube = kb.sphere_to_real(ps).cpu().numpy()
+    ps = ps.cpu().numpy()
+    for i in range(3):
+        c3 = np.zeros(n ** 3, dtype=complex)
+        c3[mp] = ps[i]
+        r = np.fft.ifftn(c3.reshape(n, n, n))
+        ref = r.reshape(-1) * (n ** 3 / np.sqrt(vol))
+        assert np.abs(cube[i] - ref).max() <= 1e-13 * np.abs(ref).max()
+        ref = np.fft.fftn(r * Vn).reshape(-1)[mp] + kn * ps[i]
+        assert np.abs(hp[i] - ref).max() <= 1e-13 * np.abs(ref).max()
+
+
+def test_full_size_properties_192():
+    """BASELINE full-size grid (192^3, the C3 cell: Si 5x5x5 supercell)."""
+    _full_size_checks(5, 192, 264859)                              # SURVEY §8 table, config C3
+
+
+def test_full_size_properties_150():
+    """The benchmark cell's grid (150^3, Si 4x4x4 supercell, the n_pw of bench.py's flagship workload)."""
+    _full_size_checks(4, 150, 135491)
 
 
 def test_against_committed_golden_fixture():

@@ -6,6 +6,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import fft_reference as fr
 from oracle.basis import Element, Model, PlaneWaveBasis
 from silicon import LATTICE, POSITIONS
 
@@ -95,6 +96,46 @@ def test_emulated_pipeline(emu, fft_size, Ecut, prefix):
     else:
         assert rc == 0
         np.testing.assert_allclose(out2, ref[:, perm], atol=1e-11 * np.abs(ref).max())
+
+
+@pytest.mark.parametrize("frac", [fr.HALF, fr.FULL], ids=["half", "full"])
+@pytest.mark.parametrize("axis", ["x", "y", "z"])
+@pytest.mark.parametrize("n", [a * b for a, b in fr.reg_pairs()])
+def test_emulated_register_engine_every_pair(emu, n, axis, frac):
+    """Every factor pair of the register engine, on each axis of an (n, 18, 25)-type box, against the direct DFT: local
+    apply, sphere -> real, real -> sphere and density, on an off-centre ellipsoid filling half or all of the box."""
+    shape = fr.placements(n)[axis]
+    nx, ny, nz = shape
+    N = nx * ny * nz
+    mapping = fr.ellipsoid_mapping(shape, frac)
+    assert frac != fr.FULL or mapping.size == N
+    npw = ctypes.c_int64(mapping.size)
+    assert emu.emur_ranges_ok(nx, ny, nz, npw, _p(mapping)) == 1
+    rng = np.random.default_rng(n)
+    nb = 2
+    psi = rng.standard_normal((nb, mapping.size)) + 1j * rng.standard_normal((nb, mapping.size))
+    V = rng.standard_normal(N)
+    kin = rng.random(mapping.size)
+    ifft_norm, fft_norm = 0.37, 1.9 / N
+
+    def check(got, ref):
+        assert np.abs(got - ref).max() <= 1e-13 * np.abs(ref).max()
+    out = np.full_like(psi, np.nan)
+    assert emu.emur_apply_local(nx, ny, nz, npw, _p(mapping), _p(psi), nb, _p(np.ascontiguousarray(V / N)), _p(kin),
+                                _p(out)) == 0
+    check(out, fr.local_apply(psi, mapping, shape, V, kin))
+    cube = np.full((nb, N), np.nan + 0j)
+    assert emu.emur_sphere_to_real(nx, ny, nz, npw, _p(mapping), _p(psi), nb, ctypes.c_double(ifft_norm), _p(cube)) == 0
+    check(cube, fr.sphere_to_real(psi, mapping, shape, ifft_norm))
+    f = rng.standard_normal((nb, N)) + 1j * rng.standard_normal((nb, N))
+    back = np.full_like(psi, np.nan)
+    assert emu.emur_real_to_sphere(nx, ny, nz, npw, _p(mapping), _p(f), nb, ctypes.c_double(fft_norm), _p(back)) == 0
+    check(back, fr.real_to_sphere(f, mapping, shape, fft_norm))
+    w = np.array([1.5, 0.0])
+    rho0 = rng.random(N)
+    rho = rho0.copy()
+    assert emu.emur_density(nx, ny, nz, npw, _p(mapping), _p(psi), nb, _p(w), _p(rho)) == 0
+    check(rho - rho0, fr.density(psi, w, mapping, shape))
 
 
 @pytest.mark.parametrize("fft_size", [(8, 9, 10), (15, 15, 15), (33, 5, 7), (40, 3, 16), (1, 4, 25)])
