@@ -111,13 +111,14 @@ static int ctx_create_common(int device, dftk_b200_ctx** out) {
   dftk_b200_ctx* c = new dftk_b200_ctx();
   c->device = device;
   c->sm_count = prop.multiProcessorCount;
+  CUDA_CHECK(cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
   c->stream = 0;  // legacy default stream: ordered with the caller's default-stream work
   CUBLAS_CHECK(cublasCreate(&c->cublas));
   CUBLAS_CHECK(cublasSetStream(c->cublas, c->stream));
   CUSOLVER_CHECK(cusolverDnCreate(&c->cusolver));
   CUSOLVER_CHECK(cusolverDnSetStream(c->cusolver, c->stream));
   fft_set_attributes();
-  reg_set_attributes();
+  reg_set_attributes(c->smem_optin);
   blas_set_attributes();
   i8tc2_set_attributes();
   lobpcg_set_attributes();
@@ -398,6 +399,36 @@ __global__ void k_scale_copy(double* dst, const double* src, double f, int64_t n
   if (i < n) dst[i] = src[i] * f;
 }
 
+// Vt[x][y][z] = f V[z][y][x]: one (z, x) tile transpose per y, coalesced on both sides
+__global__ void k_scale_transpose_xz(double* __restrict__ dst, const double* __restrict__ src, double f, int nx, int ny, int nz) {
+  __shared__ double tile[32][33];
+  const int y = blockIdx.z, x0 = blockIdx.x * 32, z0 = blockIdx.y * 32;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int z = z0 + i, x = x0 + threadIdx.x;
+    if (z < nz && x < nx) tile[i][threadIdx.x] = src[((size_t)z * ny + y) * nx + x];
+  }
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
+    const int x = x0 + i, z = z0 + threadIdx.x;
+    if (x < nx && z < nz) dst[((size_t)x * ny + y) * nz + z] = tile[threadIdx.x][i] * f;
+  }
+}
+
+// the scaled potential of a k-block or grid, and on grids with a fused y-z stage its [x][y][z] copy
+static void install_potential(dftk_b200_grid* g, const double* d, dftk::DevBuf<double>& V, dftk::DevBuf<double>& Vt) {
+  dftk_b200_ctx* ctx = g->ctx;
+  const int64_t N = g->N;
+  const double f = g->fft_norm * g->ifft_norm;
+  V.ensure(N);
+  // pre-scale by fft_normalization * ifft_normalization = 1/N (src/terms/Hamiltonian.jl:152-153)
+  LAUNCH(ctx, k_scale_copy, (unsigned)((N + 255) / 256), 256, 0, V.p, d, f, N);
+  if (grid_yz_fusable(g)) {
+    Vt.ensure(N);
+    LAUNCH(ctx, k_scale_transpose_xz, dim3((g->nx + 31) / 32, (g->nz + 31) / 32, g->ny), dim3(32, 8), 0, Vt.p, d, f, g->nx,
+           g->ny, g->nz);
+  }
+}
+
 int dftk_b200_kblock_set_potential(dftk_b200_kblock* kb, const double* V) {
   dftk_b200_ctx* ctx = kb ? kb->grid->ctx : nullptr;
   API_BEGIN
@@ -409,9 +440,7 @@ int dftk_b200_kblock_set_potential(dftk_b200_kblock* kb, const double* V) {
   }
   const int64_t N = kb->grid->N;
   const double* d = (const double*)stage_in(ctx, V, N * sizeof(double), ctx->stage_in);
-  kb->V.ensure(N);
-  // pre-scale by fft_normalization * ifft_normalization = 1/N (src/terms/Hamiltonian.jl:152-153)
-  LAUNCH(ctx, k_scale_copy, (unsigned)((N + 255) / 256), 256, 0, kb->V.p, d, kb->grid->fft_norm * kb->grid->ifft_norm, N);
+  install_potential(kb->grid, d, kb->V, kb->Vt);
   kb->has_V = true;
   API_END(ctx)
 }
@@ -426,8 +455,7 @@ int dftk_b200_grid_set_potential(dftk_b200_grid* grid, int spin, const double* V
   }
   const int64_t N = grid->N;
   const double* d = (const double*)stage_in(ctx, V, N * sizeof(double), ctx->stage_in);
-  grid->Vs[spin].ensure(N);
-  LAUNCH(ctx, k_scale_copy, (unsigned)((N + 255) / 256), 256, 0, grid->Vs[spin].p, d, grid->fft_norm * grid->ifft_norm, N);
+  install_potential(grid, d, grid->Vs[spin], grid->Vts[spin]);
   grid->has_Vs[spin] = true;
   API_END(ctx)
 }

@@ -105,6 +105,7 @@ struct dftk_b200_ctx {
   int small_dense = 1;    // LOBPCG with <= 32 bands: fused small-matrix kernels (lobpcg_small.cuh); 0 = GEMM + cuSOLVER path
   dftk::DevBuf<int> small_counter;   // arrival counter of k_small_gram (kept at zero between launches)
   int sm_count = 132;
+  int smem_optin = 227 * 1024;   // largest dynamic shared memory of one CTA (cudaDevAttrMaxSharedMemoryPerBlockOptin)
   std::string last_error;
   dftk::DevBuf<char> solver_work;
   dftk::DevBuf<int> dev_info;

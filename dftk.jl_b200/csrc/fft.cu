@@ -109,16 +109,31 @@ const RegKernels* reg_kernels_for(int n) {
     if (k.A == A && k.B == B) return &k;
   return nullptr;
 }
-void reg_set_attributes() {
-  for (const RegKernels& k : reg_table())
+void reg_set_attributes(int smem_optin) {
+  for (const RegKernels& k : reg_table()) {
     for (const void* f : {k.sphere_to_x, k.y_backward, k.z_apply, k.z_to_cube, k.z_from_cube, k.z_density,
-                          k.y_forward, k.x_to_sphere, k.z_apply_pipe, k.m_sphere_to_x, k.m_y_backward, k.m_z_apply, k.m_y_forward,
+                          k.y_forward, k.x_to_sphere, k.sphere_to_xt, k.xt_to_sphere, k.z_apply_pipe, k.m_sphere_to_x, k.m_y_backward, k.m_z_apply, k.m_y_forward,
                           k.m_x_to_sphere, k.m_z_density})
       CUDA_CHECK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem));
+    // the fused y-z stage keeps a whole y-z intermediate per CTA: it may use all the shared memory of an SM
+    CUDA_CHECK(cudaFuncSetAttribute(k.yz_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+  }
 }
 // must match RegPair<A,B>::L (fft_reg.cuh)
 static inline int reg_L(const RegKernels* k) { return k->T >= 12 ? 8 : (k->T >= 5 ? 16 : 32); }
 static inline size_t reg_smem(const RegKernels* k) { return 2 * (size_t)k->A * k->B * (reg_L(k) + 1) * sizeof(cplx); }
+// must match RegYZ<A,B>::smem on the device (fft_reg.cuh): S[n_zc][n|1] and one exchange buffer of kYzLines lines
+static const int kYzLines = 25;
+static inline size_t yz_smem(int n, int n_zc) { return ((size_t)n_zc + kYzLines) * (n | 1) * sizeof(cplx); }
+
+// The local H apply runs its y and z passes in one kernel per (band, x line) (kr_yz_apply) when y and z share a factor
+// pair of the register engine and the line's y-z intermediate fits in one CTA's shared memory.  The grid part of the
+// condition also decides whether the potential gets its [x][y][z] copy.
+bool grid_yz_fusable(const dftk_b200_grid* g) { return g->rx && g->ry && g->rz && g->ny == g->nz; }
+static bool kb_yz_fused(const dftk_b200_kblock* kb) {
+  const dftk_b200_grid* g = kb->grid;
+  return grid_yz_fusable(g) && kb->T.ranges_ok && yz_smem(g->ny, kb->Th.n_zc) <= (size_t)g->ctx->smem_optin;
+}
 static void launch_ptr(dftk_b200_ctx* ctx, const void* f, dim3 grid, int threads, size_t smem, void** args) {
   CUDA_CHECK(cudaLaunchKernel(f, grid, dim3(threads), args, smem, ctx->stream));
   ctx->launches++;
@@ -150,12 +165,12 @@ void fft_cube_inplace(dftk_b200_grid* g, cplx* data, int sign, int64_t batch) {
   }
 }
 
-int band_chunk_for(dftk_b200_kblock* kb, int64_t n_bands) {
+int band_chunk_for(dftk_b200_kblock* kb, int64_t n_bands, bool with_W2) {
   dftk_b200_grid* g = kb->grid;
   int64_t chunk = g->ctx->band_chunk;
   if (chunk <= 0) {
     // enough CTAs to fill the machine several times over, bounded scratch (<= ~4 GiB)
-    size_t per_band = ((size_t)kb->Th.n_cols * g->nx + (size_t)kb->Th.n_zc * g->ny * g->nx) * sizeof(cplx);
+    size_t per_band = ((size_t)kb->Th.n_cols * g->nx + (with_W2 ? (size_t)kb->Th.n_zc * g->ny * g->nx : 0)) * sizeof(cplx);
     chunk = (int64_t)((size_t)4 << 30) / (int64_t)(per_band ? per_band : 1);
     if (chunk > 64) chunk = 64;
     if (chunk < 1) chunk = 1;
@@ -241,10 +256,33 @@ void kb_apply_local_kinetic(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, i
     return;
   }
   REQUIRE(kb->has_V, "apply_h: local potential not set (dftk_b200_kblock_set_potential)");
-  const int chunk = band_chunk_for(kb, n_bands);
+  const bool fused = kb_yz_fused(kb);
+  const int chunk = band_chunk_for(kb, n_bands, !fused);
   for (int64_t b0 = 0; b0 < n_bands; b0 += chunk) {
     int nb = (int)std::min<int64_t>(chunk, n_bands - b0);
     const cplx* p = psi + b0 * kb->n_pw;
+    if (fused) {
+      // x-major W1 [band][x][col]: sphere -> x lines, y-z in shared memory per x line, x lines -> sphere
+      kb->W1.ensure((size_t)nb * kb->Th.n_cols * g->nx);
+      int L = reg_L(g->rx), Lp = L + 1;
+      const size_t sm_x = reg_smem(g->rx) + 5 * L * sizeof(int);
+      const cplx* twx = (const cplx*)g->twx.p;
+      const cplx* twy = (const cplx*)g->twy.p;
+      cplx* W1 = kb->W1.p;
+      int64_t ld = kb->n_pw;
+      void* a1[] = {&kb->T, &twx, &p, &ld, &W1, &L, &Lp};
+      launch_ptr(ctx, g->rx->sphere_to_xt, dim3(cdiv(kb->T.n_cols, L), nb), L * g->rx->T, sm_x, a1);
+      const double* Vt = kb->Vtp();
+      void* a2[] = {&kb->T, &twy, &W1, &Vt};
+      launch_ptr(ctx, g->ry->yz_apply, dim3(nb, g->nx), kYzLines * g->ry->T, yz_smem(g->ny, kb->T.n_zc), a2);
+      cplx* out = hpsi + b0 * kb->n_pw;
+      double scale = 1.0;
+      const double* kin = with_kin ? kb->kin.p : nullptr;
+      int acc = accumulate ? 1 : 0;
+      void* a3[] = {&kb->T, &twx, &W1, &out, &ld, &scale, &kin, &p, &ld, &acc, &L, &Lp};
+      launch_ptr(ctx, g->rx->xt_to_sphere, dim3(cdiv(kb->T.n_cols, L), nb), L * g->rx->T, sm_x, a3);
+      continue;
+    }
     kb_sphere_to_planes(kb, p, kb->n_pw, nb);
     if ((g->rz && kb->T.ranges_ok)) {
       int L = reg_L(g->rz), Lp = L + 1;

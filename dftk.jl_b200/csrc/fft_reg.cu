@@ -16,10 +16,11 @@ namespace dftk {
 extern __shared__ __align__(16) unsigned char dyn_smem_reg[];
 #define REG_MAXT(A, B) (32 * ((A) > (B) ? (A) : (B)))
 
-template <int A, int B>
+// XM: W1 layout, 0 = [col][x], 1 = [x][col] (fused y-z path)
+template <int A, int B, int XM>
 __global__ void __launch_bounds__(REG_MAXT(A, B))
 kr_sphere_to_x(SphereTablesX T, const cplx* tw, const cplx* psi, int64_t ldpsi, cplx* W1, int L, int Lp) {
-  reg_sphere_to_x<A, B>(T, tw, psi, ldpsi, W1, L, Lp, (cplx*)dyn_smem_reg, Dim3i{(int)blockIdx.x, (int)blockIdx.y, 0});
+  reg_sphere_to_x<A, B, XM>(T, tw, psi, ldpsi, W1, L, Lp, (cplx*)dyn_smem_reg, Dim3i{(int)blockIdx.x, (int)blockIdx.y, 0});
 }
 template <int A, int B>
 __global__ void __launch_bounds__(REG_MAXT(A, B))
@@ -56,12 +57,18 @@ __global__ void __launch_bounds__(REG_MAXT(A, B))
 kr_y_forward(SphereTablesX T, const cplx* tw, const cplx* W2, cplx* W1, int L, int Lp) {
   reg_y_forward<A, B>(T, tw, W2, W1, L, Lp, (cplx*)dyn_smem_reg, Dim3i{(int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z});
 }
-template <int A, int B>
+template <int A, int B, int XM>
 __global__ void __launch_bounds__(REG_MAXT(A, B))
 kr_x_to_sphere(SphereTablesX T, const cplx* tw, const cplx* W1, cplx* out, int64_t ldout, double scale,
                const double* kin, const cplx* psi, int64_t ldpsi, int accumulate, int L, int Lp) {
-  reg_x_to_sphere<A, B>(T, tw, W1, out, ldout, scale, kin, psi, ldpsi, accumulate, L, Lp, (cplx*)dyn_smem_reg,
+  reg_x_to_sphere<A, B, XM>(T, tw, W1, out, ldout, scale, kin, psi, ldpsi, accumulate, L, Lp, (cplx*)dyn_smem_reg,
                         Dim3i{(int)blockIdx.x, (int)blockIdx.y, 0});
+}
+// fused y and z passes of the local H apply (ny == nz): one CTA per (band, x line), grid (bands, nx)
+template <int A, int B>
+__global__ void __launch_bounds__(RegYZ<A, B>::LL * RegYZ<A, B>::T, 1)
+kr_yz_apply(SphereTablesX T, const cplx* tw, cplx* W1t, const double* Vt) {
+  reg_yz_apply<A, B>(T, tw, W1t, Vt, (cplx*)dyn_smem_reg, Dim3i{(int)blockIdx.y, 0, (int)blockIdx.x});
 }
 
 // ---- the same five H-apply stages for MANY k-blocks in one launch (batched small-matrix LOBPCG, lobpcg.cu): the band
@@ -127,7 +134,8 @@ static RegKernels make_entry() {
   k.A = A;
   k.B = B;
   k.T = RegPair<A, B>::T;
-  k.sphere_to_x = (const void*)kr_sphere_to_x<A, B>;
+  k.sphere_to_x = (const void*)kr_sphere_to_x<A, B, 0>;
+  k.sphere_to_xt = (const void*)kr_sphere_to_x<A, B, 1>;
   k.y_backward = (const void*)kr_y_backward<A, B>;
   k.z_apply = (const void*)kr_z_apply<A, B>;
   k.z_apply_pipe = (const void*)kr_z_apply_pipe<A, B>;
@@ -135,7 +143,9 @@ static RegKernels make_entry() {
   k.z_from_cube = (const void*)kr_z_from_cube<A, B>;
   k.z_density = (const void*)kr_z_density<A, B>;
   k.y_forward = (const void*)kr_y_forward<A, B>;
-  k.x_to_sphere = (const void*)kr_x_to_sphere<A, B>;
+  k.x_to_sphere = (const void*)kr_x_to_sphere<A, B, 0>;
+  k.xt_to_sphere = (const void*)kr_x_to_sphere<A, B, 1>;
+  k.yz_apply = (const void*)kr_yz_apply<A, B>;
   k.m_sphere_to_x = (const void*)kr_sphere_to_x_multi<A, B>;
   k.m_y_backward = (const void*)kr_y_backward_multi<A, B>;
   k.m_z_apply = (const void*)kr_z_apply_multi<A, B>;

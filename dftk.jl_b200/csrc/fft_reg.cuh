@@ -417,6 +417,138 @@ HD void reg_y_forward(const SphereTablesX& T, const cplx* __restrict__ tw, const
   }
 }
 
+// ---------------------------------------------------------------------------------------------- fused y-z stage
+// The y and z passes of the local H apply for one x line of one band (ny == nz, so both axes use the pair (A, B) and one
+// twiddle table).  The whole pruned y-z intermediate of the line, S[zc][y] (n_zc * (n|1) complex numbers), stays in
+// shared memory, so only the x-major W1 row W1t[band][x][0:n_cols] crosses global memory, once in and once out:
+//   y backward: the sphere columns of LL planes at a time -> S rows
+//   z apply:    LL y lines at a time: S[zc][y] -> inverse z transform -> * Vt(x, y, .) -> forward z transform -> S[zc][y]
+//   y forward:  LL S rows at a time -> the sphere columns of the plane, back into W1t in place
+// E[line][n|1] is the exchange buffer of every pass (the y passes read or write S / W1t on the other side); the two
+// exchanges of the z pass alias on the device as in reg_z_apply_potential.  Grid (bands, nx); blockDim == LL * T.
+// LL = 25 lines per round: fewer, fuller rounds hide more latency in the single CTA per SM (at 150^3 with 71 planes the
+// buffers take 231 936 of the H100's 232 448 bytes, and 150 y lines are exactly six rounds; 16 lines ran 15 % slower).
+template <int A, int B>
+struct RegYZ {
+  static constexpr int n = A * B, T = RegPair<A, B>::T, LL = 25, Sy = n | 1;   // odd row stride: conflict-free columns
+  static size_t smem(int n_zc) { return ((size_t)n_zc + (DFTK_Z_ALIAS ? 1 : 2) * LL) * Sy * sizeof(cplx); }
+};
+
+template <int A, int B>
+HD void reg_yz_apply(const SphereTablesX& T, const cplx* __restrict__ tw, cplx* __restrict__ W1t,
+                     const double* __restrict__ Vt, cplx* sm, Dim3i bid) {
+  constexpr int n = A * B, TT = RegYZ<A, B>::T, LL = RegYZ<A, B>::LL, Sy = RegYZ<A, B>::Sy;
+  const int n_zc = T.n_zc, x = bid.x;
+  cplx* S = sm;
+  cplx* E = sm + (size_t)n_zc * Sy;
+  cplx* E2 = DFTK_Z_ALIAS ? E : E + (size_t)LL * Sy;
+  cplx* row = W1t + ((size_t)bid.z * T.nx + x) * T.n_cols;
+  const double* vx = Vt + (size_t)x * n * n;
+  const uint64_t pol_keep = l2_policy_evict_last();
+  // y backward: planes zc0 .. zc0+LL-1
+  for (int zc0 = 0; zc0 < n_zc; zc0 += LL) {
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, zc = zc0 + line;
+      if (p < B && zc < n_zc) {
+        const PlaneCols pc = plane_cols(T, zc);
+        cplx v[A];
+#pragma unroll
+        for (int r = 0; r < A; ++r) {
+          int c = pc.col(p + B * r);
+          v[r] = ld_pred(row + (c < 0 ? 0 : c), c >= 0);
+        }
+        pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
+      }
+    }
+    TSYNC();
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, zc = zc0 + line;
+      if (p < A && zc < n_zc) {
+        cplx X[B];
+        pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
+#pragma unroll
+        for (int d = 0; d < B; ++d) S[zc * Sy + p + A * d] = X[d];
+      }
+    }
+    TSYNC();
+  }
+  // z apply: y lines y0 .. y0+LL-1 (S columns)
+  for (int y0 = 0; y0 < n; y0 += LL) {
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, y = y0 + line;
+      if (p < B && y < n) {
+        cplx v[A];
+#pragma unroll
+        for (int r = 0; r < A; ++r) {
+          int zc = zc_index(T, p + B * r);
+          v[r] = zc >= 0 ? S[zc * Sy + y] : make_double2(0.0, 0.0);
+        }
+        pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
+      }
+    }
+    TSYNC();
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, y = y0 + line;
+      cplx Y[B];
+      if (p < A && y < n) {
+        cplx X[B];
+        pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
+#pragma unroll
+        for (int d = 0; d < B; ++d) X[d] = cscale(X[d], ld_pred_hint(vx + y * n + p + A * d, true, pol_keep));
+        pass1_compute<B, A, -1>(X, p, tw, Y);
+      }
+#if DFTK_Z_ALIAS
+      __syncthreads();   // every thread of the CTA runs this body exactly once (blockDim == LL*TT)
+#endif
+      if (p < A && y < n) {
+#pragma unroll
+        for (int c = 0; c < B; ++c) E2[line * Sy + c * A + p] = Y[c];
+      }
+    }
+    TSYNC();
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, y = y0 + line;
+      if (p < B && y < n) {
+        cplx X[A];
+        pass2_load<B, A, -1>(X, p, 0, E2 + line * Sy, 1);
+#pragma unroll
+        for (int f = 0; f < A; ++f) {
+          int zc = zc_index(T, p + B * f);
+          if (zc >= 0) S[zc * Sy + y] = X[f];
+        }
+      }
+    }
+    TSYNC();
+  }
+  // y forward: planes zc0 .. zc0+LL-1, the sphere columns back to the W1t row
+  for (int zc0 = 0; zc0 < n_zc; zc0 += LL) {
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, zc = zc0 + line;
+      if (p < B && zc < n_zc) {
+        cplx v[A];
+#pragma unroll
+        for (int r = 0; r < A; ++r) v[r] = S[zc * Sy + p + B * r];
+        pass1_store<A, B, -1>(v, p, 0, E + line * Sy, 1, tw);
+      }
+    }
+    TSYNC();
+    TLOOP(t, LL * TT) {
+      const int line = t % LL, p = t / LL, zc = zc0 + line;
+      if (p < A && zc < n_zc) {
+        const PlaneCols pc = plane_cols(T, zc);
+        cplx X[B];
+        pass2_load<A, B, -1>(X, p, 0, E + line * Sy, 1);
+#pragma unroll
+        for (int d = 0; d < B; ++d) {
+          int c = pc.col(p + A * d);
+          st_pred(row + (c < 0 ? 0 : c), X[d], c >= 0);
+        }
+      }
+    }
+    TSYNC();
+  }
+}
+
 // ---------------------------------------------------------------------------------------------- x stages
 // (contiguous axis: coalesced transposing load/store through shared memory)
 // Column descriptors of the CTA's L columns, staged in shared memory: {first slot, n0, s0, n1, s1}
@@ -432,7 +564,20 @@ HD void load_col_desc(const SphereTablesX& T, int c0, int L, int* cd) {
   }
 }
 
-template <int A, int B>
+// W1 of a band is [col][x] (XM == 0: the y / z stages read x-contiguous lines) or [x][col] (XM == 1: the fused y-z
+// stage reads one x row).  The element order of the copy loops follows the layout, so consecutive threads always touch
+// consecutive addresses (for [x][col]: the L columns of the tile, 8 * 16 B = 128 B at L = 8).
+template <int n, int L, int XM>
+HD void w1_index(int t, int& line, int& x) {
+  line = XM ? t % L : t / n;
+  x = XM ? t / L : t % n;
+}
+template <int n, int XM>
+HD size_t w1_offset(int c, int x, int n_cols) {
+  return XM ? (size_t)x * n_cols + c : (size_t)c * n + x;
+}
+
+template <int A, int B, int XM = 0>
 HD void reg_sphere_to_x(const SphereTablesX& T, const cplx* __restrict__ tw, const cplx* __restrict__ psi,
                         int64_t ldpsi, cplx* __restrict__ W1, int L_rt, int Lp_rt, cplx* sm, Dim3i bid) {
   constexpr int n = A * B, TT = RegPair<A, B>::T, L = RegPair<A, B>::L, Lp = RegPair<A, B>::Lp;
@@ -479,13 +624,14 @@ HD void reg_sphere_to_x(const SphereTablesX& T, const cplx* __restrict__ tw, con
   TSYNC();
   cplx* out = W1 + (size_t)band * T.n_cols * n;
   TLOOPC(t, L * n, L * TT) {
-    int line = t / n, x = t % n;
-    int c = c0 + line;
-    if (c < T.n_cols) out[(size_t)c * n + x] = bufA[x * Lp + line];
+    int line, x;
+    w1_index<n, L, XM>(t, line, x);
+    const int c = c0 + line;
+    if (c < T.n_cols) out[w1_offset<n, XM>(c, x, T.n_cols)] = bufA[x * Lp + line];
   }
 }
 
-template <int A, int B>
+template <int A, int B, int XM = 0>
 HD void reg_x_to_sphere(const SphereTablesX& T, const cplx* __restrict__ tw, const cplx* __restrict__ W1,
                         cplx* __restrict__ out, int64_t ldout, double scale, const double* __restrict__ kin,
                         const cplx* __restrict__ psi, int64_t ldpsi, int accumulate, int L_rt, int Lp_rt, cplx* sm,
@@ -501,9 +647,10 @@ HD void reg_x_to_sphere(const SphereTablesX& T, const cplx* __restrict__ tw, con
   const cplx* in = W1 + (size_t)band * T.n_cols * n;
   load_col_desc(T, c0, L, cd);
   TLOOPC(t, L * n, L * TT) {
-    int line = t / n, x = t % n;
-    int c = c0 + line;
-    bufA[x * Lp + line] = (c < T.n_cols) ? in[(size_t)c * n + x] : make_double2(0.0, 0.0);
+    int line, x;
+    w1_index<n, L, XM>(t, line, x);
+    const int c = c0 + line;
+    bufA[x * Lp + line] = (c < T.n_cols) ? in[w1_offset<n, XM>(c, x, T.n_cols)] : make_double2(0.0, 0.0);
   }
   TSYNC();
   TLOOP(t, L * TT) {

@@ -41,7 +41,7 @@ HD cplx ld_pred(const cplx* p, bool ok) {
 #endif
 }
 // L2 eviction policies: the potential V(r) (N_fft doubles, re-read by every band) should stay resident in the
-// 126 MB L2 while the per-band pruned intermediates stream through it once.
+// 50 MB L2 of the H100 while the per-band pruned intermediates stream through it once.
 HD uint64_t l2_policy_evict_last() {
 #if defined(__CUDA_ARCH__)
   uint64_t pol;

@@ -11,6 +11,8 @@ struct RegKernels {
   int A, B, T;
   const void *sphere_to_x, *y_backward, *z_apply, *z_to_cube, *z_from_cube, *z_density, *y_forward, *x_to_sphere;
   const void* z_apply_pipe;   // persistent, software-pipelined form of z_apply (cp.async staged input tiles)
+  const void* yz_apply;       // fused y-z stage of the local H apply on an x-major W1 (ny == nz)
+  const void *sphere_to_xt, *xt_to_sphere;   // the x stages on the x-major W1 of yz_apply
   const void *m_sphere_to_x, *m_y_backward, *m_z_apply, *m_y_forward, *m_x_to_sphere, *m_z_density;   // many k-blocks per launch
 };
 // one k-block's share of a batched H-apply launch (local + kinetic part)
@@ -27,7 +29,7 @@ struct FftMultiItem {
   int nb;
 };
 const RegKernels* reg_kernels_for(int n);   // nullptr: use the generic Stockham engine
-void reg_set_attributes();
+void reg_set_attributes(int smem_optin);
 }  // namespace dftk
 
 namespace dftk {
@@ -50,6 +52,7 @@ struct dftk_b200_grid {
   int Lx, Ly, Lz;
   const dftk::RegKernels *rx = nullptr, *ry = nullptr, *rz = nullptr;  // register engine per axis
   dftk::DevBuf<double> Vs[2];   // total local potential per spin (pre-scaled by 1/N), shared by the k-blocks that opt in
+  dftk::DevBuf<double> Vts[2];  // the same as [x][y][z] (z contiguous) for the fused y-z stage, when the grid has one
   bool has_Vs[2] = {false, false};
 };
 
@@ -79,6 +82,8 @@ struct dftk_b200_kblock {
   bool has_V = false;
   int grid_V = -1;                // >= 0: use grid->Vs[grid_V] instead of the block's own copy
   const double* Vp() const { return grid_V >= 0 ? grid->Vs[grid_V].p : V.p; }
+  dftk::DevBuf<double> Vt;        // V as [x][y][z], written beside V on grids with a fused y-z stage (grid_yz_fusable)
+  const double* Vtp() const { return grid_V >= 0 ? grid->Vts[grid_V].p : Vt.p; }
   // scratch
   dftk::DevBuf<dftk::cplx> W1, W2;    // pruned intermediates for a chunk of bands
   dftk::DevBuf<dftk::cplx> proj;      // n_proj x n_bands (+ D*proj)
@@ -91,7 +96,8 @@ struct dftk_b200_kblock {
 
 namespace dftk {
 // fft.cu
-int band_chunk_for(dftk_b200_kblock* kb, int64_t n_bands);
+int band_chunk_for(dftk_b200_kblock* kb, int64_t n_bands, bool with_W2 = true);
+bool grid_yz_fusable(const dftk_b200_grid* g);
 void fft_cube_inplace(dftk_b200_grid* g, cplx* data, int sign, int64_t batch);
 void kb_sphere_to_planes(dftk_b200_kblock* kb, const cplx* psi, int64_t ldpsi, int nb);
 void kb_planes_to_sphere(dftk_b200_kblock* kb, cplx* out, int64_t ldout, int nb, double scale,
