@@ -379,6 +379,7 @@ int dftk_b200_kblock_create(dftk_b200_grid* grid, int64_t n_pw, const int64_t* m
         kb->PD.ensure((size_t)n_pw * n_proj);
         zgemm(ctx, 0, n_pw, n_proj, n_proj, make_double2(1, 0), kb->P.p, n_pw, kb->Dc.p, n_proj, make_double2(0, 0), kb->PD.p, n_pw);
       }
+      kb_setup_fold(kb, map_h.data());
     }
     CUDA_CHECK(cudaStreamSynchronize(s));
   } catch (...) {
@@ -478,6 +479,7 @@ int dftk_b200_kblock_trim(dftk_b200_kblock* kb) {
   kb->W1.release();
   kb->W2.release();
   kb->proj.release();
+  kb->fold_ws.release();
   API_END(ctx)
 }
 
@@ -582,7 +584,7 @@ int dftk_b200_band_energies(dftk_b200_kblock* kb, const void* psi, int64_t n_ban
       cplx* proj = kb->proj.ensure((size_t)2 * np * n_bands);
       cplx* dproj = proj + (size_t)np * n_bands;
       const cplx one = make_double2(1, 0), zero = make_double2(0, 0);
-      zgemm(ctx, 2, np, n_bands, kb->n_pw, one, kb->P.p, kb->n_pw, d, kb->n_pw, zero, proj, np);
+      kb_project(kb, d, n_bands, proj);
       zgemm(ctx, 0, np, n_bands, np, one, kb->Dc.p, np, proj, np, zero, dproj, np);
       LAUNCH(ctx, k_nonlocal_band_energy, (unsigned)((n_bands + 63) / 64), 64, 0, (const cplx*)proj,
              (const cplx*)dproj, np, n_bands, sc + n_bands);

@@ -78,6 +78,12 @@ struct dftk_b200_kblock {
   dftk::DevBuf<signed char> i8_planes;   // gemm_backend 4: cached INT8 residue planes of P (built at first use)
   dftk::DevBuf<int> i8_exps;
   dftk::DevBuf<dftk::cplx> PD;    // P D (n_pw x n_proj), kept when n_proj is small: Hψ += (P D)(P'ψ) as two batched small products
+  // time-reversal fold of the projector products (blas.cu, kb_setup_fold): set on blocks whose sphere is closed under
+  // q -> -q and whose projectors satisfy P(-q) = conj(P(q)); n_half = 0 keeps the complex products
+  int64_t n_half = 0;                   // |H|: one plane wave of each pair ±q
+  dftk::DevBuf<int> fold_i, fold_p;     // H (ascending sphere indices) and the partner -q of each
+  dftk::DevBuf<double> R;               // [Re P(H); Im P(H)]: 2 n_half x n_proj, column-major
+  dftk::DevBuf<dftk::cplx> fold_ws;     // folded orbitals, then [a; b], for a chunk of bands (2 n_half x chunk)
   dftk::DevBuf<double> V;         // N, pre-scaled by 1/N (fft_norm*ifft_norm)
   bool has_V = false;
   int grid_V = -1;                // >= 0: use grid->Vs[grid_V] instead of the block's own copy
@@ -124,6 +130,9 @@ void zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_t k, cplx
 //             transA == 0 -> B is upper triangular (trmm-like: half the flops)
 void blas_set_attributes();
 void kb_apply_nonlocal(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_t n_bands);
+void kb_project(dftk_b200_kblock* kb, const cplx* psi, int64_t n_bands, cplx* proj);   // proj = P' psi (n_proj x n_bands)
+bool sphere_mirror(int nx, int ny, int nz, int64_t n_pw, const int64_t* map, std::vector<int>& mir);
+void kb_setup_fold(dftk_b200_kblock* kb, const int64_t* map_h);
 void columnwise_dots(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
                      int64_t n_rows, int64_t n_cols, cplx* out_dev);
 void kin_dots(dftk_b200_ctx* ctx, const cplx* X, int64_t ldx, const double* kin, int64_t n_rows,
