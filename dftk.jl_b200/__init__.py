@@ -59,7 +59,7 @@ from . import _lib
 from ._lib import DftkB200Error, LIB_PATH
 from .device import Context, FFTGrid, KBlock
 from .architecture import B200, CPU
-from .pseudo import PspHgh, ElementPsp, load_psp, parse_hgh
+from .pseudo import PspHgh, PspUpf, ElementPsp, load_psp, parse_hgh, parse_upf
 from .model import Model, model_DFT, model_atomic, LDA, PBE, SymOp, symmetry_operations
 from .parallel import KpointComm, split_evenly
 from .basis import PlaneWaveBasis, MonkhorstPack, ExplicitKpoints, Kpoint, compute_fft_size

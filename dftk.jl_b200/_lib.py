@@ -60,6 +60,7 @@ SIGNATURES = {
     "dftk_b200_ewald": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_dbl, c_vp, c_vp, c_vp, c_vp]),
     "dftk_b200_structure_factor": (c_int, [c_vp, c_int, c_vp, c_vp, c_vp]),
     "dftk_b200_build_projectors": (c_int, [c_vp, c_i64, c_vp, c_int, c_vp, c_int, c_vp, c_vp]),
+    "dftk_b200_radial_transform": (c_int, [c_vp, c_i64, c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "dftk_b200_columnwise_dots": (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp]),
     "dftk_b200_tall_gram": (c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp]),
     "dftk_b200_zgemm": (c_int, [c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp,

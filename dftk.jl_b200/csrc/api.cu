@@ -812,6 +812,19 @@ int dftk_b200_build_projectors(dftk_b200_ctx* ctx, int64_t n_pw, const double* g
   API_END(ctx)
 }
 
+int dftk_b200_radial_transform(dftk_b200_ctx* ctx, int64_t n_r, const double* r, int n_f, const double* g, const int32_t* l,
+                               int64_t n_q, const double* q, double* F) {
+  API_BEGIN
+  REQUIRE(ctx && n_r >= 1 && n_f >= 0 && n_q >= 0 && (n_f == 0 || n_q == 0 || (r && g && l && q && F)),
+          "radial_transform: bad argument");
+  if (n_f > 0 && n_q > 0) {
+    REQUIRE(is_device_ptr(r) && is_device_ptr(g) && is_device_ptr(q) && is_device_ptr(F) && !is_device_ptr(l),
+            "radial_transform: r, g, q and F on the device, l on the host");
+    radial_transform(ctx, n_r, r, n_f, g, (const int*)l, n_q, q, F);
+  }
+  API_END(ctx)
+}
+
 // ------------------------------------------------------------------ dense helpers
 int dftk_b200_columnwise_dots(dftk_b200_ctx* ctx, const void* A, const void* B, int64_t n_rows,
                               int64_t n_cols, void* out_host) {

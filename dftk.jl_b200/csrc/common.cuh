@@ -113,6 +113,7 @@ struct dftk_b200_ctx {
   dftk::DevBuf<char> gemm_ws;    // split-K partials
   dftk::DevBuf<int> sym_i;       // symmetry tables (integer rotations)
   dftk::DevBuf<double> sym_d;    //                 (fractional translations)
+  dftk::DevBuf<double> radial_part;   // per-split partial sums of the radial transform (setup.cu)
   dftk::DevBuf<char> stage_in, stage_out;  // host<->device staging for host-buffer calls
   // pipelined host staging (H2D of chunk k+1 || compute of chunk k || D2H of chunk k-1)
   cudaStream_t s_in = nullptr, s_out = nullptr;

@@ -170,6 +170,13 @@ void ewald(dftk_b200_ctx* ctx, const double* lattice_colmajor, int n_atoms, cons
 void structure_factor(dftk_b200_grid* g, int n_atoms, const double* pos_host, const double* coeff_host, cplx* out);
 void build_projectors(dftk_b200_ctx* ctx, int64_t n_pw, const double* gpk, int n_atoms, const double* pos_host, int n_rows,
                       const cplx* ff, cplx* P);
+constexpr int RADIAL_MAX_F = 16;     // functions per launch of the radial transform (accumulators held in registers)
+struct RadialL {                     // angular momenta of the functions of one launch, passed by value
+  int l[RADIAL_MAX_F];
+  int lmax;
+};
+void radial_transform(dftk_b200_ctx* ctx, int64_t n_r, const double* r, int n_f, const double* g, const int* l_host, int64_t n_q,
+                      const double* q, double* F);
 // lobpcg.cu
 int lobpcg_run(dftk_b200_kblock* kb, cplx* X, int64_t M, double tol, int miniter, int maxiter,
                int64_t n_conv_check, bool use_prec, double* lambda_host, double* resid_host,

@@ -5,8 +5,9 @@ The two terms that touch grid-sized or orbital-sized data run in libdftk_b200:
   * local:    one kernel pass over the cube per atom (dftk_b200_local_forces),
   * nonlocal: four tensor-core projections P†[ψ, p_x ψ, p_y ψ, p_z ψ] per k-block give the forces on every atom at once
               (dftk_b200_nonlocal_force_rows) instead of the reference's 3·n_atoms full-height GEMM pairs.
-Ewald forces are O(n_atoms²) host arithmetic.  Kinetic, Hartree, Xc (the HGH tables carry no non-linear core
-correction), PspCorrection and Entropy do not contribute.  Forces are in reduced coordinates like the reference;
+Ewald forces are O(n_atoms²) host arithmetic.  Xc contributes only through a model core density (non-linear core
+correction of a UPF pseudopotential, xc.jl:206-260); its contraction is that of the local term and uses the same kernel.
+Kinetic, Hartree, PspCorrection and Entropy do not contribute.  Forces are in reduced coordinates like the reference;
 `compute_forces_cart` converts.
 """
 import math
@@ -29,6 +30,32 @@ def forces_local(basis, rho):
     for group in model.atom_groups:
         ff = model.atoms[group[0]].psp.eval_psp_local_fourier(pn)
         w = (torch.conj(rho_f) * ff / math.sqrt(model.unit_cell_volume)).contiguous()
+        pos = np.ascontiguousarray(np.array([model.positions[i] for i in group], dtype=np.float64))
+        out = np.zeros((len(group), 3))
+        check(ctx.L.dftk_b200_local_forces(basis.fft_grid.h, _ptr(w), len(group), _ptr(pos), _ptr(out)), ctx.h)
+        for j, ia in enumerate(group):
+            F[ia] = F[ia] + out[j]
+    return F
+
+
+def forces_xc(basis, rho):
+    """compute_forces(::TermXc), xc.jl:206-260: the force of the non-linear core correction,
+    F_a,α = -Re Σ_G -2πi G_α e^{-2πi G·r_a} conj(V̄xc(G)) ρ̂core(|G|) / sqrt(Ω) with V̄xc the spin average of the xc potential
+    at ρ + ρcore -- the contraction of the local-potential force, so it runs through the same kernel.  None without ρcore."""
+    model = basis.model
+    term = basis.term("Xc")
+    if term is None or term.rho_core is None:
+        return None
+    ctx = basis.architecture.ctx
+    _, pot = term.potential(basis, rho)
+    v_f = basis.fft(pot.mean(dim=0)).reshape(-1)
+    pn = basis.G_vectors_cart.norm(dim=1)
+    F = [np.zeros(3) for _ in model.positions]
+    for group in model.atom_groups:
+        psp = model.atoms[group[0]].psp
+        if not getattr(psp, "has_core_density", False):
+            continue
+        w = (torch.conj(v_f) * psp.eval_psp_core_density_fourier(pn) / math.sqrt(model.unit_cell_volume)).contiguous()
         pos = np.ascontiguousarray(np.array([model.positions[i] for i in group], dtype=np.float64))
         out = np.zeros((len(group), 3))
         check(ctx.L.dftk_b200_local_forces(basis.fft_grid.h, _ptr(w), len(group), _ptr(pos), _ptr(out)), ctx.h)
@@ -191,6 +218,10 @@ def compute_forces(basis_or_scfres, psi=None, occupation=None, *, rho=None, per_
         elif name == "Ewald":
             parts[name] = energy_forces_ewald_device(basis.architecture.ctx, model.lattice, [a.charge_ionic() for a in model.atoms],
                                                      model.positions)[1]
+        elif name == "Xc":
+            f = forces_xc(basis, rho)
+            if f is not None:
+                parts[name] = f
     total = [sum((p[i] for p in parts.values()), np.zeros(3)) for i in range(len(model.positions))]
     return (total, parts) if per_term else total
 

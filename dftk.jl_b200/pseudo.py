@@ -1,6 +1,8 @@
-"""Analytic GTH/HGH pseudopotentials for the host-side setup (mirror of src/pseudo/PspHgh.jl and
-src/elements.jl ElementPsp).  Setup code: runs once per basis, vectorised with torch on the device."""
+"""Pseudopotentials for the host-side setup: analytic GTH/HGH (mirror of src/pseudo/PspHgh.jl), numerical
+norm-conserving UPF (src/pseudo/PspUpf.jl) and src/elements.jl ElementPsp.  Setup code: runs once per basis,
+vectorised with torch on the device; the UPF radial transforms are a CUDA kernel."""
 import math
+import os
 import re
 import numpy as np
 import torch
@@ -21,7 +23,7 @@ _TABLE = {
                      (0.22285578, [[-12.38579937]])]),
 }
 _ATOMIC_NUMBER = {"H": 1, "He": 2, "Li": 3, "C": 6, "N": 7, "O": 8, "Na": 11, "Mg": 12, "Al": 13, "Si": 14,
-                  "Fe": 26, "Cu": 29}
+                  "Fe": 26, "Cu": 29, "Tl": 81}
 
 
 class PspHgh:
@@ -110,7 +112,236 @@ def parse_hgh(text, identifier=""):
     return PspHgh(sum(n_elec), rloc, cloc, rp, h, identifier)
 
 
+def _simpson_weights(x, uniform):
+    """Quadrature weights of src/common/quadrature.jl (simpson_uniform / simpson_nonuniform, with the end correction for an
+    odd number of intervals; trapezoidal below five points) on the nodes x."""
+    n = len(x)
+    w = np.zeros(n)
+    if n == 1:
+        return w
+    if n <= 4 or uniform is None:
+        w[0] = (x[1] - x[0]) / 2
+        w[1:n - 1] = (x[2:] - x[:n - 2]) / 2
+        w[n - 1] += (x[n - 1] - x[n - 2]) / 2
+        return w
+    odd = (n - 1) % 2 == 1
+    if uniform:
+        dx = x[1] - x[0]
+        istop = n - 2 if odd else n - 1                   # last node (1-based) of the composite part
+        w[0] = dx / 3
+        w[1:istop:2] = 4 / 3 * dx                          # 1-based even nodes
+        w[2:istop:2] = 2 / 3 * dx
+        if odd:
+            w[n - 1] += 5 / 12 * dx
+            w[n - 2] += dx
+            w[n - 3] -= dx / 12
+        else:
+            w[n - 1] += dx / 3
+        return w
+    m = n - 1 if odd else n                               # composite panels over the first m nodes
+    dx0, dx1 = x[1:m:2] - x[0:m - 1:2], x[2:m:2] - x[1:m - 1:2]
+    c = (dx0 + dx1) / 6
+    np.add.at(w, np.arange(0, m - 2, 2), c * (2 - dx1 / dx0))
+    np.add.at(w, np.arange(1, m - 1, 2), c * (dx0 + dx1) ** 2 / (dx0 * dx1))
+    np.add.at(w, np.arange(2, m, 2), c * (2 - dx0 / dx1))
+    if odd:
+        dxn, dxm = x[-1] - x[-2], x[-2] - x[-3]
+        w[n - 1] += (2 * dxn ** 2 + 3 * dxn * dxm) / (6 * (dxm + dxn))
+        w[n - 2] += (dxn ** 2 + 3 * dxn * dxm) / (6 * dxm)
+        w[n - 3] -= dxn ** 3 / (6 * dxm * (dxm + dxn))
+    return w
+
+
+class PspUpf:
+    """Numerical norm-conserving pseudopotential read from a UPF v2 file (src/pseudo/PspUpf.jl).  Stored as in the
+    reference: vloc in Ha, r²β per projector cut at its cutoff_radius_index, h[l] = 2·PP_DIJ, r²ρion = PP_RHOATOM/4π,
+    r²ρcore = r²·PP_NLCC.  The Fourier-space form factors are radial transforms evaluated on the device
+    (dftk_b200_radial_transform), once per distinct |q| of a call."""
+
+    def __init__(self, Zion, lmax, rgrid, vloc, r2_projs, h, r2_rhoion, r2_rhocore, r2_taucore, identifier="",
+                 description=""):
+        self.Zion, self.lmax = int(Zion), int(lmax)
+        self.rgrid = np.ascontiguousarray(rgrid, dtype=np.float64)
+        self.vloc = np.asarray(vloc, dtype=np.float64)
+        self.r2_projs = [[np.asarray(f, dtype=np.float64) for f in fl] for fl in r2_projs]
+        self.h = [np.array(x, dtype=float) for x in h]
+        self.r2_rhoion = np.asarray(r2_rhoion, dtype=np.float64)
+        self.r2_rhocore = np.asarray(r2_rhocore, dtype=np.float64)
+        self.r2_taucore = np.asarray(r2_taucore, dtype=np.float64)     # read and kept; meta-GGA is not supported
+        self.rcut = float(self.rgrid[-1])
+        self.identifier, self.description = identifier, description
+        # default_psp_quadrature: the rule is chosen on the full mesh, (x2-x1) ≈ (x3-x2) with Julia's rtol √eps, atol 0
+        r = self.rgrid
+        if len(r) <= 4:
+            self._uniform = None
+        else:
+            a, b = r[1] - r[0], r[2] - r[1]
+            self._uniform = bool(abs(a - b) <= math.sqrt(np.finfo(float).eps) * max(abs(a), abs(b)))
+        self._tables = {}
+        self._cache = (None, None)
+
+    def count_n_proj_radial(self, l):
+        return self.h[l].shape[0]
+
+    def count_n_proj(self):
+        return sum((2 * l + 1) * self.h[l].shape[0] for l in range(self.lmax + 1))
+
+    @property
+    def has_core_density(self):
+        return bool(np.any(self.r2_rhocore != 0))
+
+    @property
+    def has_valence_density(self):
+        return bool(np.any(self.r2_rhoion != 0))
+
+    def weights(self, n):
+        """Quadrature weights of the first n mesh points (each function is integrated over its own length)."""
+        return _simpson_weights(self.rgrid[:n], self._uniform)
+
+    def _table(self, kind, device):
+        """(r, g, l) on the device for one group of functions: g = weights · r²f, zero-padded to the mesh length."""
+        key = (kind, str(device))
+        if key not in self._tables:
+            r, n = self.rgrid, len(self.rgrid)
+            if kind == "proj":
+                rows, ls = [], []
+                for l in range(self.lmax + 1):
+                    for f in self.r2_projs[l]:
+                        g = np.zeros(n)
+                        g[:len(f)] = self.weights(len(f)) * f
+                        rows.append(g)
+                        ls.append(l)
+            elif kind == "local":        # l = 0 transform of r²(vloc + Z erf(r)/r): the smooth part of PspUpf.jl:229-242
+                rows, ls = [self.weights(n) * r * (r * self.vloc + self.Zion * _erf(r))], [0]
+            elif kind == "core":
+                rows, ls = [self.weights(n) * self.r2_rhocore], [0]
+            elif kind == "valence":
+                rows, ls = [self.weights(n) * self.r2_rhoion], [0]
+            g = torch.from_numpy(np.ascontiguousarray(np.array(rows).reshape(len(rows), n))).to(device)
+            self._tables[key] = (torch.from_numpy(r).to(device), g, np.ascontiguousarray(ls, dtype=np.int32))
+        return self._tables[key]
+
+    def radial_transform(self, kind, p):
+        """F[f, :] for every function of `kind` at the |q| values p (torch, float64): the kernel runs on the distinct
+        values only and the result is gathered back."""
+        from ._lib import lib, check
+        from .device import _ptr
+        r, g, ls = self._table(kind, p.device)
+        flat = p.reshape(-1).contiguous()
+        uq, inv = torch.unique(flat, return_inverse=True)
+        uq = uq.contiguous()
+        F = torch.empty((len(ls), uq.numel()), dtype=torch.float64, device=p.device)
+        h = _radial_ctx(p.device)
+        check(lib().dftk_b200_radial_transform(h, len(r), _ptr(r), len(ls), _ptr(g), _ptr(ls), uq.numel(), _ptr(uq), _ptr(F)), h)
+        return F[:, inv].reshape((len(ls),) + tuple(p.shape))
+
+    def eval_psp_projector_fourier(self, i, l, p):
+        # build_projector_form_factors asks for every (l, i) at the same |G+k|: one launch serves all projectors of the
+        # pseudopotential, and the rows are kept while the caller holds on to that tensor
+        if self._cache[0] is not p:
+            self._cache = (p, self.radial_transform("proj", p))
+        row = sum(self.count_n_proj_radial(ll) for ll in range(l)) + i - 1
+        return self._cache[1][row]
+
+    def eval_psp_local_fourier(self, p):
+        F = self.radial_transform("local", p)[0]
+        safe = torch.where(p == 0, torch.ones_like(p), p)
+        F = F - 4 * math.pi * self.Zion * torch.exp(-safe * safe / 4) / (safe * safe)
+        return torch.where(p == 0, torch.zeros_like(F), F)
+
+    def eval_psp_core_density_fourier(self, p):
+        return self.radial_transform("core", p)[0]
+
+    def eval_psp_valence_density_fourier(self, p):
+        return self.radial_transform("valence", p)[0]
+
+    def eval_psp_energy_correction(self):
+        r = self.rgrid
+        return 4 * math.pi * float(np.sum(self.weights(len(r)) * r * (r * self.vloc + self.Zion)))
+
+
+def _erf(x):
+    from scipy.special import erf
+    return erf(x)
+
+
+def _radial_ctx(device):
+    """The library context of the GPU that holds p: the one a basis on that device already uses, else the context
+    B200(device) would create."""
+    from .architecture import B200
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    for c in B200._contexts.values():
+        if c.device.index == idx:
+            return c.h
+    return B200(device=idx).ctx.h
+
+
+def _upf_values(node):
+    return np.array(node.text.split(), dtype=float)
+
+
+def parse_upf(text, identifier=""):
+    """UPF v2 (XML) reader with the unit conversions of PspUpf.jl:97-158."""
+    import xml.etree.ElementTree as ET
+    if not re.search(r"<UPF\s+version\s*=\s*\"2", text[:4096]):
+        raise ValueError("UPF: only version 2 (XML) files are supported")
+    root = ET.fromstring(text)
+    hd = root.find("PP_HEADER")
+    flag = lambda k: hd.get(k, "F").strip().upper() in ("T", "TRUE", ".TRUE.")
+    ptype = hd.get("pseudo_type", "").strip()
+    unsupported = []
+    if flag("has_so"):
+        unsupported.append("spin-orbit coupling")
+    if ptype == "SL":
+        unsupported.append("semilocal potential")
+    if ptype in ("US", "USPP"):
+        unsupported.append("ultrasoft")
+    if ptype == "PAW":
+        unsupported.append("projector-augmented wave")
+    if flag("has_gipaw"):
+        unsupported.append("gipaw data")
+    if ptype == "1/r":
+        unsupported.append("Coulomb")
+    if unsupported:
+        raise ValueError("Pseudopotential contains the following unsupported features/quantities: " + ",".join(unsupported))
+    lmax = int(hd.get("l_max"))
+    if lmax > 3:
+        raise ValueError(f"UPF: l_max = {lmax} > 3 is not supported (solid harmonics stop at l = 3)")
+    rgrid = _upf_values(root.find("PP_MESH").find("PP_R"))
+    n = len(rgrid)
+    vloc = _upf_values(root.find("PP_LOCAL"))[:n] / 2                   # Ry -> Ha
+    nl = root.find("PP_NONLOCAL")
+    betas = [b for b in nl if b.tag.startswith("PP_BETA")] if nl is not None else []
+    nb = len(betas)
+    dij = _upf_values(nl.find("PP_DIJ")).reshape(nb, nb) * 2 if nb else np.zeros((0, 0))    # 1/Ry -> 1/Ha
+    ang = [int(b.get("angular_momentum")) for b in betas]
+    r2_projs, h = [], []
+    for l in range(lmax + 1):
+        idx = [i for i in range(nb) if ang[i] == l]
+        fl = []
+        for i in idx:
+            cut = int(betas[i].get("cutoff_radius_index", str(n)))
+            fl.append(rgrid[:cut] * (_upf_values(betas[i])[:cut] / 2))        # rβ (Ry) -> r²β (Ha)
+        r2_projs.append(fl)
+        h.append(dij[np.ix_(idx, idx)])
+    opt = lambda tag: root.find(tag)
+    rho = opt("PP_RHOATOM")
+    r2_rhoion = _upf_values(rho)[:n] / (4 * math.pi) if rho is not None else np.zeros(n)
+    nlcc = opt("PP_NLCC")
+    r2_rhocore = rgrid ** 2 * _upf_values(nlcc)[:n] if nlcc is not None else np.zeros(n)
+    tau = opt("PP_TAUMOD")
+    r2_taucore = rgrid ** 2 * _upf_values(tau)[:n] if tau is not None else np.zeros(n)
+    return PspUpf(round(float(hd.get("z_valence"))), lmax, rgrid, vloc, r2_projs, h, r2_rhoion, r2_rhocore, r2_taucore,
+                  identifier=identifier, description=(hd.get("comment") or "").strip())
+
+
 def load_psp(symbol, functional="lda"):
+    """load_psp(symbol, functional): the built-in GTH tables; load_psp(path): a .upf, .hgh or .gth file."""
+    ext = os.path.splitext(str(symbol))[1].lower()
+    if ext in (".upf", ".hgh", ".gth"):
+        with open(symbol) as fh:
+            text = fh.read()
+        return parse_upf(text, identifier=str(symbol)) if ext == ".upf" else parse_hgh(text, identifier=str(symbol))
     Z, n_elec, rloc, cloc, proj = _TABLE[(symbol, functional)]
     rp, h = [], []
     for r, rows in proj:

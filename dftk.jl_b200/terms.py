@@ -298,13 +298,35 @@ class TermHartree:
         return E, [RealSpaceMultiplication(basis, k, pot) for k in basis.kpoints]
 
 
+def core_density(basis):
+    """ρcore of the non-linear core correction (xc.jl:30-40): the superposition of the model core densities of every
+    species that has one, split equally over the spin components (ρ_from_total), not renormalised.  None if no species
+    has a core density."""
+    model = basis.model
+    groups = [g for g in model.atom_groups if getattr(model.atoms[g[0]].psp, "has_core_density", False)]
+    if not groups:
+        return None
+    pn = basis.G_vectors_cart.norm(dim=1)
+    rho = torch.zeros(basis.N, dtype=torch.complex128, device=pn.device)
+    for group in groups:
+        ff = model.atoms[group[0]].psp.eval_psp_core_density_fourier(pn)
+        rho += structure_factor(basis, [model.positions[i] for i in group]) * ff / math.sqrt(model.unit_cell_volume)
+    rtot = basis.irfft(basis.enforce_real(rho)).reshape(-1)
+    n_spin = model.n_spin_components
+    return (rtot[None, :] if n_spin == 1 else torch.stack([rtot / 2, rtot / 2])).contiguous()
+
+
 class TermXc:
-    """xc.jl:84-160 (LDA / GGA; potential = Vρ - 2 ∇·(Vσ ∇ρ))."""
+    """xc.jl:84-160 (LDA / GGA; potential = Vρ - 2 ∇·(Vσ ∇ρ)).  With a model core density (NLCC) the energy and the
+    potential are evaluated at ρ + ρcore (gradients included); the potential is still the derivative with respect to ρ."""
 
     def __init__(self, basis):
         self.functionals = list(basis.model.functionals)
+        self.rho_core = core_density(basis)
 
     def potential(self, basis, rho):
+        if self.rho_core is not None:
+            rho = rho + self.rho_core
         n_spin = rho.shape[0]
         is_gga = any(f.startswith("gga") for f in self.functionals)
         sigma = grad = None
@@ -419,17 +441,26 @@ def build_kblocks(basis):
 
 
 def guess_density(basis, magnetic_moments=None):
-    """density_methods.jl:103-181,237-244: superposition of Gaussian valence densities."""
+    """density_methods.jl:103-181,237-244 with ValenceDensityAuto: superposition of atomic valence densities, the
+    pseudo-atomic one (PP_RHOATOM) for species whose pseudopotential has it, a Gaussian for every other species."""
     model = basis.model
     pn = basis.G_vectors_cart.norm(dim=1)
     Gf = basis.G_vectors.to(torch.float64)
+    form_factors = {}
+
+    def form_factor(a0):
+        if a0 not in form_factors:
+            if getattr(a0.psp, "has_valence_density", False):
+                form_factors[a0] = a0.psp.eval_psp_valence_density_fourier(pn)
+            else:
+                L = atom_decay_length(a0.n_elec_core(), a0.n_elec_valence())
+                form_factors[a0] = a0.charge_ionic() * torch.exp(-(pn * L) ** 2)
+        return form_factors[a0]
 
     def superposition(coeffs):
         rho = torch.zeros(basis.N, dtype=torch.complex128, device=pn.device)
         for group in model.atom_groups:
-            a0 = model.atoms[group[0]]
-            L = atom_decay_length(a0.n_elec_core(), a0.n_elec_valence())
-            ff = a0.charge_ionic() * torch.exp(-(pn * L) ** 2)
+            ff = form_factor(model.atoms[group[0]])
             sf = structure_factor(basis, [model.positions[i] for i in group], [coeffs[i] for i in group])
             rho += sf * ff / math.sqrt(model.unit_cell_volume)
         return basis.irfft(basis.enforce_real(rho)).reshape(-1)

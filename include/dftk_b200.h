@@ -225,6 +225,13 @@ int dftk_b200_structure_factor(dftk_b200_grid* grid, int n_atoms, const double* 
  * (device); P: (n_atoms·n_rows) × n_pw complex, i.e. the column-major n_pw × n_proj block of these atoms (device). */
 int dftk_b200_build_projectors(dftk_b200_ctx* ctx, int64_t n_pw, const double* gpk, int n_atoms, const double* positions,
                                int n_rows, const void* form_factors, void* P);
+/* Radial (modified Hankel) transforms of n_f functions tabulated on one radial mesh (the eval_psp_*_fourier methods of a
+ * numerical UPF pseudopotential, src/pseudo/PspUpf.jl, src/common/hankel.jl):
+ *   F[f, q] = 4π / q^l_f · Σ_i g[f, i] j_{l_f}(q r_i),   and for q <= 10·eps the limit 4π/(2l_f+1)!! · Σ_i g[f, i] r_i^l_f.
+ * r: n_r mesh points (device); g: n_f × n_r row-major integrands r²f(r) times the quadrature weights, zero beyond the end of a
+ * function (device); l: n_f angular momenta 0..3 (host); q: n_q values >= 0 (device); F: n_f × n_q row-major (device). */
+int dftk_b200_radial_transform(dftk_b200_ctx* ctx, int64_t n_r, const double* r, int n_f, const double* g, const int32_t* l,
+                               int64_t n_q, const double* q, double* F);
 
 /* ---- small dense helpers used by the host driver (columnwise_dots, src/common/linalg.jl:2-15) ---- */
 int dftk_b200_columnwise_dots(dftk_b200_ctx* ctx, const void* A, const void* B, int64_t n_rows,
