@@ -70,6 +70,8 @@ from .occupation import compute_occupation
 from .densities import compute_density, symmetrize_rho
 from .forces import (compute_forces, compute_forces_cart, symmetrize_forces, energy_forces_ewald,
                      energy_forces_ewald_device)
+from .hubbard import (OrbitalManifold, Hubbard, TermHubbard, atomic_orbital_projectors, atomic_orbital_projections,
+                      compute_hubbard_n, symmetrize_hubbard_n, wigner_d_matrix, resolve_hubbard_manifold)
 from .scf import (self_consistent_field, next_density, AdaptiveBands, FixedBands, AdaptiveDiagtol,
                   ScfConvergenceDensity, ScfConvergenceEnergy, SimpleMixing, KerkerMixing, LdosMixing, compute_ldos,
                   AndersonAcceleration, ScfDefaultCallback)

@@ -34,6 +34,10 @@ SIGNATURES = {
     "dftk_b200_fft_cube": (c_int, [c_vp, c_vp, c_int, c_i64]),
     "dftk_b200_kblock_create": (c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_dbl, P(c_vp)]),
     "dftk_b200_kblock_destroy": (c_int, [c_vp]),
+    "dftk_b200_kblock_set_orbitals": (c_int, [c_vp, c_i64, c_vp]),
+    "dftk_b200_kblock_set_orbital_coefficients": (c_int, [c_vp, c_vp]),
+    "dftk_b200_kblock_fold_size": (c_int, [c_vp, P(c_i64)]),
+    "dftk_b200_orbital_occupation_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "dftk_b200_kblock_set_potential": (c_int, [c_vp, c_vp]),
     "dftk_b200_grid_set_potential": (c_int, [c_vp, c_int, c_vp]),
     "dftk_b200_kblock_use_grid_potential": (c_int, [c_vp, c_int]),

@@ -234,7 +234,7 @@ class PlaneWaveBasis:
         return self.Gplusk_vectors(kpt) @ self._recip.T
 
     def term(self, name):
-        for n, t in zip(self.model.term_types, self.terms):
+        for n, t in zip(self.model.term_names, self.terms):
             if n == name:
                 return t
         return None

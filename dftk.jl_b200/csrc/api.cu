@@ -333,6 +333,7 @@ int dftk_b200_kblock_create(dftk_b200_grid* grid, int64_t n_pw, const int64_t* m
     kb->spin = spin;
     kb->kweight = kweight;
     kb->Th = build_sphere_tables(grid->nx, grid->ny, grid->nz, n_pw, map_h.data());
+    kb->map_h = map_h;
     const SphereTablesHost& H = kb->Th;
     cudaStream_t s = ctx->stream;
     kb->d_col_start.upload(H.col_start.data(), H.col_start.size(), s);
@@ -393,6 +394,89 @@ int dftk_b200_kblock_create(dftk_b200_grid* grid, int64_t n_pw, const int64_t* m
 int dftk_b200_kblock_destroy(dftk_b200_kblock* kb) {
   delete kb;
   return DFTK_B200_OK;
+}
+
+int dftk_b200_kblock_set_orbitals(dftk_b200_kblock* kb, int64_t n_orb, const void* Phi) {
+  dftk_b200_ctx* ctx = kb ? kb->grid->ctx : nullptr;
+  API_BEGIN
+  REQUIRE(kb && n_orb >= 0 && (n_orb == 0 || Phi), "kblock_set_orbitals: bad argument");
+  const int64_t n_pw = kb->n_pw, np = kb->n_proj, n = np + n_orb;
+  cudaStream_t s = ctx->stream;
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  {
+    // the new table [P | Φ]; the old one is freed when `old` leaves this scope (after the stream has drained)
+    DevBuf<cplx> old;
+    std::swap(old.p, kb->P.p);
+    std::swap(old.cap, kb->P.cap);
+    if (n > 0) {
+      kb->P.ensure((size_t)n_pw * n);
+      if (np) CUDA_CHECK(cudaMemcpyAsync(kb->P.p, old.p, (size_t)n_pw * np * sizeof(cplx), cudaMemcpyDeviceToDevice, s));
+      if (n_orb)
+        CUDA_CHECK(cudaMemcpyAsync(kb->P.p + n_pw * np, Phi, (size_t)n_pw * n_orb * sizeof(cplx), cudaMemcpyDefault, s));
+    }
+    kb->n_orb = n_orb;
+    if (n_orb) {
+      // D of the H apply: [D 0; 0 V] with V = 0 until kblock_set_orbital_coefficients
+      kb->Dh.ensure((size_t)n * n);
+      CUDA_CHECK(cudaMemsetAsync(kb->Dh.p, 0, (size_t)n * n * sizeof(cplx), s));
+      if (np)
+        CUDA_CHECK(cudaMemcpy2DAsync(kb->Dh.p, n * sizeof(cplx), kb->Dc.p, np * sizeof(cplx), np * sizeof(cplx), np,
+                                     cudaMemcpyDeviceToDevice, s));
+    } else {
+      kb->Dh.release();
+    }
+    if (n > 0 && n <= 96) {      // SMALL_MAX_COLS of the batched small-matrix path (lobpcg_small.cuh)
+      kb->PD.ensure((size_t)n_pw * n);
+      kb_refresh_pd(kb, 0);
+    } else {
+      kb->PD.release();
+    }
+    // the INT8 planes of gemm_backend 4 describe the old table: prepared again at first use
+    kb->i8_Pop = I8Operand{};
+    // Löwdin keeps Φ(-q) = conj Φ(q) at time-reversal-invariant k (S is real there); checked like the projectors
+    kb_setup_fold(kb, kb->map_h.data());
+    CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  API_END(ctx)
+}
+
+int dftk_b200_kblock_fold_size(dftk_b200_kblock* kb, int64_t* n_half) {
+  dftk_b200_ctx* ctx = kb ? kb->grid->ctx : nullptr;
+  API_BEGIN
+  REQUIRE(kb && n_half, "kblock_fold_size: NULL argument");
+  *n_half = kb->n_half;
+  API_END(ctx)
+}
+
+int dftk_b200_kblock_set_orbital_coefficients(dftk_b200_kblock* kb, const void* V) {
+  dftk_b200_ctx* ctx = kb ? kb->grid->ctx : nullptr;
+  API_BEGIN
+  REQUIRE(kb, "kblock_set_orbital_coefficients: kblock is NULL");
+  REQUIRE(kb->n_orb > 0, "kblock_set_orbital_coefficients: the k-block has no orbitals (kblock_set_orbitals)");
+  const int64_t np = kb->n_proj, no = kb->n_orb, n = np + no;
+  cudaStream_t s = ctx->stream;
+  cplx* blk = kb->Dh.p + np + n * np;
+  if (V)
+    CUDA_CHECK(cudaMemcpy2DAsync(blk, n * sizeof(cplx), V, no * sizeof(cplx), no * sizeof(cplx), no, cudaMemcpyDefault, s));
+  else
+    CUDA_CHECK(cudaMemset2DAsync(blk, n * sizeof(cplx), 0, no * sizeof(cplx), no));
+  kb_refresh_pd(kb, np);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  API_END(ctx)
+}
+
+int dftk_b200_orbital_occupation_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* psi,
+                                       const double* occ_w_host, int64_t ld_w, const int32_t* n_bands, void* n_out) {
+  dftk_b200_ctx* ctx = (n_blocks > 0 && kbs && kbs[0]) ? kbs[0]->grid->ctx : nullptr;
+  API_BEGIN
+  REQUIRE(n_blocks >= 0 && (n_blocks == 0 || (kbs && psi && occ_w_host && n_bands && n_out)),
+          "orbital_occupation_multi: bad argument");
+  if (n_blocks == 0) return DFTK_B200_OK;
+  REQUIRE(is_device_ptr(n_out), "orbital_occupation_multi: n_out must be device memory");
+  for (int64_t i = 0; i < n_blocks; ++i)
+    REQUIRE(kbs[i] && psi[i] && is_device_ptr(psi[i]), "orbital_occupation_multi: orbitals must be device memory");
+  orbital_occupation_multi(n_blocks, kbs, (const cplx* const*)psi, occ_w_host, ld_w, (const int*)n_bands, (cplx*)n_out);
+  API_END(ctx)
 }
 
 __global__ void k_scale_copy(double* dst, const double* src, double f, int64_t n) {
@@ -545,7 +629,7 @@ int dftk_b200_apply_terms(dftk_b200_kblock* kb, const void* psi, void* hpsi, int
 
 int dftk_b200_apply_h(dftk_b200_kblock* kb, const void* psi, void* hpsi, int64_t n_bands) {
   if (!kb) return record(nullptr, DFTK_B200_EINVAL, "apply_h: kblock is NULL");
-  int parts = (kb->has_V ? 1 : 0) | (kb->has_kin ? 2 : 0) | (kb->n_proj > 0 ? 4 : 0);
+  int parts = (kb->has_V ? 1 : 0) | (kb->has_kin ? 2 : 0) | (kb->n_nl() > 0 ? 4 : 0);
   return dftk_b200_apply_terms(kb, psi, hpsi, n_bands, parts, 0);
 }
 

@@ -840,11 +840,15 @@ __global__ void k_unfold_acc(const cplx* __restrict__ Y, int64_t ldy, const int*
   o[p] = cadd(o[p], make_double2(a.x + b.y, a.y - b.x));
 }
 
-// Pairs the sphere and checks the projectors of a new k-block; on success keeps H, the partners and R so that
-// kb_apply_nonlocal and the band energies take the folded path.  Any other block keeps the complex products.
+// Pairs the sphere and checks the projector table (atomic projectors and orbital columns) of a k-block; on success keeps
+// H, the partners and R so that kb_apply_nonlocal and the band energies take the folded path.  Any other block keeps the
+// complex products.  Called again whenever the table changes (kblock_set_orbitals).
 void kb_setup_fold(dftk_b200_kblock* kb, const int64_t* map_h) {
   kb->n_half = 0;
-  if (kb->n_proj == 0) return;
+  kb->fold_i.release();
+  kb->fold_p.release();
+  kb->R.release();
+  if (kb->n_nl() == 0) return;
   dftk_b200_ctx* ctx = kb->grid->ctx;
   const dftk_b200_grid* g = kb->grid;
   std::vector<int> mir;
@@ -855,7 +859,7 @@ void kb_setup_fold(dftk_b200_kblock* kb, const int64_t* map_h) {
       hi.push_back((int)i);
       hp.push_back(mir[i]);
     }
-  const int64_t nh = (int64_t)hi.size(), np = kb->n_proj;
+  const int64_t nh = (int64_t)hi.size(), np = kb->n_nl();
   cudaStream_t s = ctx->stream;
   kb->fold_i.upload(hi.data(), nh, s);
   kb->fold_p.upload(hp.data(), nh, s);
@@ -912,28 +916,42 @@ static void rgemm_nn(dftk_b200_ctx* ctx, int64_t Krows, int64_t n, int64_t m, co
 
 static bool kb_folds(const dftk_b200_kblock* kb) { return kb->n_half > 0 && kb->grid->ctx->gemm_backend == 0; }
 
-// proj (n_proj x n_bands) = P' psi
-void kb_project(dftk_b200_kblock* kb, const cplx* psi, int64_t n_bands, cplx* proj) {
+// proj (nc x n_bands) = P[:, c0 : c0+nc]' psi
+void kb_project_cols(dftk_b200_kblock* kb, int64_t c0, int64_t nc, const cplx* psi, int64_t n_bands, cplx* proj) {
   dftk_b200_ctx* ctx = kb->grid->ctx;
-  const int64_t np = kb->n_proj, nh = kb->n_half, kf = 2 * nh;
+  const int64_t nh = kb->n_half, kf = 2 * nh;
   if (!kb_folds(kb)) {
-    zgemm(ctx, 2, np, n_bands, kb->n_pw, make_double2(1, 0), kb->P.p, kb->n_pw, psi, kb->n_pw, make_double2(0, 0), proj, np);
+    zgemm(ctx, 2, nc, n_bands, kb->n_pw, make_double2(1, 0), kb->P.p + kb->n_pw * c0, kb->n_pw, psi, kb->n_pw,
+          make_double2(0, 0), proj, nc);
     return;
   }
-  const int64_t nc = fold_chunk(n_bands);
-  cplx* F = kb->fold_ws.ensure((size_t)kf * nc);
-  for (int64_t j0 = 0; j0 < n_bands; j0 += nc) {
-    const int64_t w = std::min(nc, n_bands - j0);
+  const int64_t w0 = fold_chunk(n_bands);
+  cplx* F = kb->fold_ws.ensure((size_t)kf * w0);
+  for (int64_t j0 = 0; j0 < n_bands; j0 += w0) {
+    const int64_t w = std::min(w0, n_bands - j0);
     LAUNCH(ctx, k_fold, (unsigned)((nh * w + 255) / 256), 256, 0, psi + kb->n_pw * j0, kb->n_pw,
            (const int*)kb->fold_i.p, (const int*)kb->fold_p.p, nh, w, F, kf);
-    rgemm_cn(ctx, np, w, kf, kb->R.p, kf, F, kf, proj + np * j0, np);
+    rgemm_cn(ctx, nc, w, kf, kb->R.p + kf * c0, kf, F, kf, proj + nc * j0, nc);
   }
+}
+
+// proj (n_proj x n_bands) = P' psi over the atomic projectors
+void kb_project(dftk_b200_kblock* kb, const cplx* psi, int64_t n_bands, cplx* proj) {
+  kb_project_cols(kb, 0, kb->n_proj, psi, n_bands, proj);
+}
+
+// PD[:, c0:] = P Dnl[:, c0:]; Dnl is block diagonal, so columns from a block boundary on only need those rows of Dnl
+void kb_refresh_pd(dftk_b200_kblock* kb, int64_t c0) {
+  const int64_t n = kb->n_nl();
+  if (!kb->PD.p || c0 >= n) return;
+  zgemm(kb->grid->ctx, 0, kb->n_pw, n - c0, n - c0, make_double2(1, 0), kb->P.p + kb->n_pw * c0, kb->n_pw,
+        kb->Dnl() + c0 + n * c0, n, make_double2(0, 0), kb->PD.p + kb->n_pw * c0, kb->n_pw);
 }
 
 // the nonlocal apply on the folded operands, one band chunk at a time; the update writes [a; b] over the folded orbitals
 static void kb_apply_nonlocal_folded(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_t n_bands) {
   dftk_b200_ctx* ctx = kb->grid->ctx;
-  const int64_t np = kb->n_proj, nh = kb->n_half, kf = 2 * nh;
+  const int64_t np = kb->n_nl(), nh = kb->n_half, kf = 2 * nh;
   const int64_t nc = fold_chunk(n_bands);
   cplx* F = kb->fold_ws.ensure((size_t)kf * nc);
   cplx* proj = kb->proj.ensure((size_t)2 * np * nc);
@@ -944,22 +962,23 @@ static void kb_apply_nonlocal_folded(dftk_b200_kblock* kb, const cplx* psi, cplx
     LAUNCH(ctx, k_fold, blocks, 256, 0, psi + kb->n_pw * j0, kb->n_pw, (const int*)kb->fold_i.p,
            (const int*)kb->fold_p.p, nh, w, F, kf);
     rgemm_cn(ctx, np, w, kf, kb->R.p, kf, F, kf, proj, np);
-    zgemm(ctx, 0, np, w, np, make_double2(1, 0), kb->Dc.p, np, proj, np, make_double2(0, 0), dproj, np);
+    zgemm(ctx, 0, np, w, np, make_double2(1, 0), kb->Dnl(), np, proj, np, make_double2(0, 0), dproj, np);
     rgemm_nn(ctx, kf, w, np, kb->R.p, kf, dproj, np, F, kf);
     LAUNCH(ctx, k_unfold_acc, blocks, 256, 0, (const cplx*)F, kf, (const int*)kb->fold_i.p, (const int*)kb->fold_p.p,
            nh, w, hpsi + kb->n_pw * j0, kb->n_pw);
   }
 }
 
-// hpsi += P (D (P' psi))      (apply!(::NonlocalOperator), src/terms/operators.jl:126-128)
+// hpsi += P (D (P' psi))      (apply!(::NonlocalOperator), src/terms/operators.jl:126-128); with Hubbard orbitals
+// attached P = [P | Φ] and D = [D 0; 0 V], so the orbital term rides in the same pair of products
 void kb_apply_nonlocal(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_t n_bands) {
-  if (kb->n_proj == 0 || n_bands == 0) return;
+  if (kb->n_nl() == 0 || n_bands == 0) return;
   if (kb_folds(kb)) {
     kb_apply_nonlocal_folded(kb, psi, hpsi, n_bands);
     return;
   }
   dftk_b200_ctx* ctx = kb->grid->ctx;
-  const int64_t np = kb->n_proj;
+  const int64_t np = kb->n_nl();
   cplx* proj = kb->proj.ensure((size_t)2 * np * n_bands);
   cplx* dproj = proj + (size_t)np * n_bands;
   const cplx one = make_double2(1.0, 0.0), zero = make_double2(0.0, 0.0);
@@ -969,12 +988,12 @@ void kb_apply_nonlocal(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_
     if (!kb->i8_Pop.planes) kb->i8_Pop = i8_prepare(ctx, kb->P.p, kb->n_pw, np, kb->n_pw, kb->i8_planes, kb->i8_exps);
     const I8Operand op_psi = i8_prepare(ctx, psi, kb->n_pw, n_bands, kb->n_pw, kb->i8_psi_planes, kb->i8_psi_exps);
     i8_gram(ctx, kb->i8_Pop, op_psi, proj, np, false);
-    zgemm(ctx, 0, np, n_bands, np, one, kb->Dc.p, np, proj, np, zero, dproj, np);
+    zgemm(ctx, 0, np, n_bands, np, one, kb->Dnl(), np, proj, np, zero, dproj, np);
     i8_update(ctx, 1, &kb->i8_Pop, dproj, np, n_bands, hpsi, kb->n_pw, 1.0, 1.0);
     return;
   }
   zgemm(ctx, 2, np, n_bands, kb->n_pw, one, kb->P.p, kb->n_pw, psi, kb->n_pw, zero, proj, np);
-  zgemm(ctx, 0, np, n_bands, np, one, kb->Dc.p, np, proj, np, zero, dproj, np);
+  zgemm(ctx, 0, np, n_bands, np, one, kb->Dnl(), np, proj, np, zero, dproj, np);
   zgemm(ctx, 0, kb->n_pw, n_bands, np, one, kb->P.p, kb->n_pw, dproj, np, one, hpsi, kb->n_pw);
 }
 

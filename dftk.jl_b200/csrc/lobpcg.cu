@@ -604,28 +604,28 @@ struct BatchExec {
         for (Op* o : ops) {
           const ApplyHItem& a = o->u.applyh;
           dftk_b200_kblock* kb = a.kb;
-          if (kb->n_proj == 0) continue;
-          if (kb->n_proj > SMALL_MAX_COLS || a.ncols > SMALL_MAX_N || !kb->PD.p) {
+          if (kb->n_nl() == 0) continue;
+          if (kb->n_nl() > SMALL_MAX_COLS || a.ncols > SMALL_MAX_N || !kb->PD.p) {
             kb_apply_nonlocal(kb, a.in, a.out, a.ncols);
             continue;
           }
-          cplx* proj = kb->proj.ensure((size_t)2 * kb->n_proj * SMALL_MAX_N);
+          cplx* proj = kb->proj.ensure((size_t)2 * kb->n_nl() * SMALL_MAX_N);
           GramItem gi{};
           gi.A.n = gi.B.n = 1;
-          gi.A.p[0] = kb->P.p; gi.A.ld[0] = kb->n_pw; gi.A.cols[0] = (int)kb->n_proj;
+          gi.A.p[0] = kb->P.p; gi.A.ld[0] = kb->n_pw; gi.A.cols[0] = (int)kb->n_nl();
           gi.B.p[0] = a.in; gi.B.ld[0] = kb->n_pw; gi.B.cols[0] = a.ncols;
-          for (int q = 1; q < 4; ++q) { gi.A.start[q] = (int)kb->n_proj; gi.B.start[q] = a.ncols; }
+          for (int q = 1; q < 4; ++q) { gi.A.start[q] = (int)kb->n_nl(); gi.B.start[q] = a.ncols; }
           gi.n_rows = kb->n_pw;
           small_gram_geometry(ctx, kb->n_pw, &gi.n_ctas, &gi.rows_per_cta);
           gi.upper_only = 0;
           gi.C = proj;
-          gi.ldc = kb->n_proj;
+          gi.ldc = kb->n_nl();
           g.push_back(gi);
           BtimesItem bi{};
           bi.Y.n = 1;
-          bi.Y.p[0] = kb->PD.p; bi.Y.ld[0] = kb->n_pw; bi.Y.cols[0] = (int)kb->n_proj;
-          for (int q = 1; q < 4; ++q) bi.Y.start[q] = (int)kb->n_proj;
-          bi.cm = proj; bi.ldcm = kb->n_proj; bi.ncols = a.ncols;
+          bi.Y.p[0] = kb->PD.p; bi.Y.ld[0] = kb->n_pw; bi.Y.cols[0] = (int)kb->n_nl();
+          for (int q = 1; q < 4; ++q) bi.Y.start[q] = (int)kb->n_nl();
+          bi.cm = proj; bi.ldcm = kb->n_nl(); bi.ncols = a.ncols;
           bi.out = a.out; bi.ldo = kb->n_pw; bi.n_rows = kb->n_pw; bi.alpha = 1.0; bi.beta = 1.0;
           b.push_back(bi);
         }
@@ -1408,7 +1408,7 @@ void Lobpcg::body(SolveArgs& a) {
       return;
     }
     touch(out);
-    flops += 16.0 * (double)(slab ? Nfull : N) * kb->n_proj * (slab ? (double)in.cols / ctx->nranks : (double)in.cols);
+    flops += 16.0 * (double)(slab ? Nfull : N) * kb->n_nl() * (slab ? (double)in.cols / ctx->nranks : (double)in.cols);
     if (slab) return apply_h_slab(in, out);
     kb_apply_local_kinetic(kb, in.p, out.p, in.cols, kb->has_V, kb->has_kin, false);
     kb_apply_nonlocal(kb, in.p, out.p, in.cols);
@@ -1601,7 +1601,7 @@ static void run_batched(dftk_b200_ctx* ctx, std::vector<Lobpcg>& L, std::vector<
   // synchronisation bubble of a round hide behind the other group's kernels (and small kernels of the two streams overlap).
   bool pipelined = ctx->batch_pipeline != 0 && n_blocks >= 8;
   for (auto& l : L)      // blocks whose nonlocal term would take the large (context-workspace) path stay in one group
-    pipelined = pipelined && (l.kb->n_proj == 0 || (l.kb->n_proj <= SMALL_MAX_COLS && l.kb->PD.p != nullptr));
+    pipelined = pipelined && (l.kb->n_nl() == 0 || (l.kb->n_nl() <= SMALL_MAX_COLS && l.kb->PD.p != nullptr));
   const int G = pipelined ? 2 : 1;
   cudaStream_t user = ctx->stream;
   if (pipelined) {
@@ -1844,6 +1844,82 @@ void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* co
   for (auto& sct : scatter) memcpy(sct.first, exec.gather_h + sct.second.first, sct.second.second * sizeof(double));
 }
 
+struct OrbOccItem { const cplx* a; int nb, spin; const double* w; };
+
+// n[s](i, j) += Σ_blocks of spin s Σ_b w_b a_ib conj(a_jb): one thread per output entry, the blocks and bands summed in
+// a fixed order (the result does not depend on scheduling)
+__global__ void k_orbital_occupation(const OrbOccItem* __restrict__ items, int n_items, int n_orb, int n_spin,
+                                     cplx* __restrict__ n_out) {
+  const int64_t nn = (int64_t)n_orb * n_orb;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n_spin * nn) return;
+  const int s = (int)(idx / nn), i = (int)(idx % nn % n_orb), j = (int)(idx % nn / n_orb);
+  double re = 0.0, im = 0.0;
+  for (int t = 0; t < n_items; ++t) {
+    const OrbOccItem it = items[t];
+    if (it.spin != s) continue;
+    for (int b = 0; b < it.nb; ++b) {
+      const cplx x = it.a[i + (int64_t)n_orb * b], y = it.a[j + (int64_t)n_orb * b];
+      const double w = it.w[b];
+      re += w * (x.x * y.x + x.y * y.y);
+      im += w * (x.y * y.x - x.x * y.y);
+    }
+  }
+  n_out[idx] = make_double2(n_out[idx].x + re, n_out[idx].y + im);
+}
+
+// Occupation matrices of the Hubbard orbitals over ALL k-blocks of a rank (hubbard.jl:201-232 before its mpi_sum):
+// a = Φ' ψ per block, then the weighted Hermitian update into the block's spin channel.  Blocks of <= 32 bands and
+// <= 96 orbitals share one batched projection launch; larger ones project with the block's own GEMMs (folded where it
+// folds).  One launch for the update and one synchronisation in all.
+void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* const* psi, const double* occ_w_host,
+                              int64_t ld_w, const int* n_bands, cplx* n_out) {
+  if (n <= 0) return;
+  dftk_b200_ctx* ctx = kbs[0]->grid->ctx;
+  const int64_t n_orb = kbs[0]->n_orb;
+  REQUIRE(n_orb > 0, "orbital_occupation_multi: the k-blocks have no orbitals (kblock_set_orbitals)");
+  BatchExec exec(ctx);
+  if (ctx->small_counter.cap < (size_t)std::max<int64_t>(n, 256)) exec.reset_counters((size_t)n);
+  // the weights get a buffer of their own: the descriptor ring is recycled whenever it fills up
+  DevBuf<double>& wbuf = kbs[0]->wts;
+  wbuf.upload(occ_w_host, (size_t)n * ld_w, ctx->stream);
+  const double* w_dev = wbuf.p;
+  std::vector<GramItem> gr;
+  std::vector<OrbOccItem> items;
+  int n_spin = 1;
+  for (int64_t i = 0; i < n; ++i) {
+    dftk_b200_kblock* kb = kbs[i];
+    const int nb = n_bands[i];
+    REQUIRE(kb && kb->grid->ctx == ctx && kb->n_orb == n_orb && nb >= 0 && nb <= ld_w,
+            "orbital_occupation_multi: bad block (all blocks need the same number of orbitals)");
+    if (nb == 0) continue;
+    n_spin = std::max(n_spin, kb->spin + 1);
+    cplx* a = kb->proj.ensure((size_t)n_orb * std::max(nb, SMALL_MAX_N));
+    if (nb <= SMALL_MAX_N && n_orb <= SMALL_MAX_COLS) {
+      GramItem g{};
+      g.A.n = g.B.n = 1;
+      g.A.p[0] = kb->P.p + kb->n_pw * kb->n_proj; g.A.ld[0] = kb->n_pw; g.A.cols[0] = (int)n_orb;
+      g.B.p[0] = psi[i]; g.B.ld[0] = kb->n_pw; g.B.cols[0] = nb;
+      for (int q = 1; q < 4; ++q) { g.A.start[q] = (int)n_orb; g.B.start[q] = nb; }
+      g.n_rows = kb->n_pw;
+      BatchExec::small_gram_geometry(ctx, kb->n_pw, &g.n_ctas, &g.rows_per_cta);
+      g.C = a;
+      g.ldc = n_orb;
+      gr.push_back(g);
+    } else {
+      kb_project_cols(kb, kb->n_proj, n_orb, psi[i], nb, a);
+    }
+    items.push_back(OrbOccItem{a, nb, kb->spin, w_dev + i * ld_w});
+  }
+  if (!gr.empty()) exec.gram_batch(gr);
+  if (!items.empty()) {
+    const int64_t total = n_spin * n_orb * n_orb;
+    LAUNCH(ctx, k_orbital_occupation, (unsigned)((total + 255) / 256), 256, 0, exec.upload(items), (int)items.size(),
+           (int)n_orb, n_spin, n_out);
+  }
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
 // C (nA x nB, host, column-major) = A' B for tall column-major blocks (n_rows >> nA, nB <= SMALL_MAX_COLS): one fused launch
 // (CTA partials + last-CTA reduction, lobpcg_small.cuh).  Used by the host driver for the history dot products of Anderson
 // mixing (src/scf/anderson.jl:81-130) instead of a QR factorisation of the N_fft x m history matrix.
@@ -1877,6 +1953,7 @@ int lobpcg_run_slab(dftk_b200_kblock* kb, cplx* Xfull, int64_t M, double tol, in
                     double* exchange_bytes) {
   dftk_b200_ctx* ctx = kb->grid->ctx;
   REQUIRE(ctx->nccl != nullptr, "lobpcg_slab: the context has no communicator (use ctx_create_dist)");
+  REQUIRE(kb->n_orb == 0, "lobpcg_slab: k-blocks with Hubbard orbitals (kblock_set_orbitals) are not supported by the slab solver");
   const int R = ctx->nranks, me = ctx->rank;
   const int64_t Nf = kb->n_pw;
   Lobpcg L;

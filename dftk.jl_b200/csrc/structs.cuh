@@ -67,9 +67,16 @@ struct dftk_b200_kblock {
       d_cx_n1;
   dftk::DevBuf<double> kin;       // n_pw (may be empty)
   bool has_kin = false;
-  dftk::DevBuf<dftk::cplx> P;     // n_pw x n_proj
+  dftk::DevBuf<dftk::cplx> P;     // n_pw x n_nl(): the atomic projectors, then the orbital columns (kblock_set_orbitals)
   std::vector<double> D_host;     // n_proj x n_proj
   dftk::DevBuf<dftk::cplx> Dc;    // complex copy of D on the device (n_proj x n_proj)
+  // Hubbard orbitals: n_orb more columns of P that every H apply carries in the same pair of projector products.
+  // n_proj, Dc, the band energies and the force rows keep covering the atomic projectors only.
+  int64_t n_orb = 0;
+  dftk::DevBuf<dftk::cplx> Dh;    // n_nl() x n_nl() block-diagonal [D 0; 0 V] of the H apply (only when n_orb > 0)
+  std::vector<int64_t> map_h;     // sphere mapping, kept to re-pair the fold when the projector table changes
+  int64_t n_nl() const { return n_proj + n_orb; }
+  const dftk::cplx* Dnl() const { return n_orb ? Dh.p : Dc.p; }
   dftk::DevBuf<signed char> i8_pool[8];  // gemm_backend 4: residue planes of the LOBPCG blocks (cache slots of a solve)
   dftk::DevBuf<int> i8_epool[8];
   dftk::I8Operand i8_Pop;                // prepared projector table (kept for the lifetime of the block)
@@ -77,12 +84,12 @@ struct dftk_b200_kblock {
   dftk::DevBuf<int> i8_psi_exps;
   dftk::DevBuf<signed char> i8_planes;   // gemm_backend 4: cached INT8 residue planes of P (built at first use)
   dftk::DevBuf<int> i8_exps;
-  dftk::DevBuf<dftk::cplx> PD;    // P D (n_pw x n_proj), kept when n_proj is small: Hψ += (P D)(P'ψ) as two batched small products
+  dftk::DevBuf<dftk::cplx> PD;    // P Dnl (n_pw x n_nl), kept when n_nl is small: Hψ += (P D)(P'ψ) as two batched small products
   // time-reversal fold of the projector products (blas.cu, kb_setup_fold): set on blocks whose sphere is closed under
   // q -> -q and whose projectors satisfy P(-q) = conj(P(q)); n_half = 0 keeps the complex products
   int64_t n_half = 0;                   // |H|: one plane wave of each pair ±q
   dftk::DevBuf<int> fold_i, fold_p;     // H (ascending sphere indices) and the partner -q of each
-  dftk::DevBuf<double> R;               // [Re P(H); Im P(H)]: 2 n_half x n_proj, column-major
+  dftk::DevBuf<double> R;               // [Re P(H); Im P(H)]: 2 n_half x n_nl, column-major
   dftk::DevBuf<dftk::cplx> fold_ws;     // folded orbitals, then [a; b], for a chunk of bands (2 n_half x chunk)
   dftk::DevBuf<double> V;         // N, pre-scaled by 1/N (fft_norm*ifft_norm)
   bool has_V = false;
@@ -131,6 +138,9 @@ void zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_t k, cplx
 void blas_set_attributes();
 void kb_apply_nonlocal(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, int64_t n_bands);
 void kb_project(dftk_b200_kblock* kb, const cplx* psi, int64_t n_bands, cplx* proj);   // proj = P' psi (n_proj x n_bands)
+// proj (nc x n_bands) = P[:, c0 : c0+nc]' psi, on the folded operands where the block has them
+void kb_project_cols(dftk_b200_kblock* kb, int64_t c0, int64_t nc, const cplx* psi, int64_t n_bands, cplx* proj);
+void kb_refresh_pd(dftk_b200_kblock* kb, int64_t c0);   // PD[:, c0:] = P Dnl[:, c0:] (PD is kept when n_nl <= 96)
 bool sphere_mirror(int nx, int ny, int nz, int64_t n_pw, const int64_t* map, std::vector<int>& mir);
 void kb_setup_fold(dftk_b200_kblock* kb, const int64_t* map_h);
 void columnwise_dots(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, const cplx* B, int64_t ldb,
@@ -190,6 +200,8 @@ int lobpcg_run_slab(dftk_b200_kblock* kb, cplx* Xfull, int64_t M, double tol, in
 void random_orbitals_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, cplx* const* Xs, int64_t M, uint64_t seed);
 void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* const* psi, const int* n_bands, int64_t ld_out,
                          double* ekin_host, double* enl_host);
+void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* const* psi, const double* occ_w_host,
+                              int64_t ld_w, const int* n_bands, cplx* n_out);
 void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
                cplx* out_host);
 void lobpcg_set_attributes();

@@ -175,6 +175,27 @@ def density_accumulate_multi(kblocks, psis, weights, rho):
     return rho
 
 
+def orbital_occupation_multi(kblocks, psis, weights, n_spin, n_orb):
+    """dftk_b200_orbital_occupation_multi: Σ_blocks Σ_n w_n (Φ'ψ_n)(Φ'ψ_n)' per spin channel over the Hubbard orbitals of
+    the k-blocks.  psis[i]: (nb_i, n_pw_i) contiguous device tensors, weights[i]: nb_i host numbers.  Returns a
+    (n_spin, n_orb, n_orb) complex host array."""
+    n = len(kblocks)
+    out = torch.zeros((n_spin, n_orb, n_orb), dtype=torch.complex128,
+                      device=kblocks[0].ctx.device if n else "cpu")
+    if n == 0:
+        return out.numpy()
+    ctx = kblocks[0].ctx
+    nbs = np.array([len(w) for w in weights], dtype=np.int32)
+    ld = max(1, int(nbs.max()))
+    w = np.zeros((n, ld))
+    for i, wi in enumerate(weights):
+        w[i, :len(wi)] = wi
+    kb_arr = (c_vp * n)(*[kb.h.value for kb in kblocks])
+    x_arr = (c_vp * n)(*[p.data_ptr() for p in psis])
+    check(ctx.L.dftk_b200_orbital_occupation_multi(n, kb_arr, x_arr, _ptr(w), ld, _ptr(nbs), _ptr(out)), ctx.h)
+    return out.cpu().numpy().transpose(0, 2, 1).copy()     # column-major per spin -> n[s, i, j]
+
+
 def random_orbitals_multi(kblocks, n_bands, seed):
     """dftk_b200_random_orbitals: orthonormal random start vectors (n_bands, n_pw_i) for a list of k-blocks."""
     n = len(kblocks)
@@ -269,6 +290,28 @@ class KBlock:
 
     def _new(self, nb):
         return torch.empty((nb, self.n_pw), dtype=torch.complex128, device=self.ctx.device)
+
+    def set_orbitals(self, Phi):
+        """dftk_b200_kblock_set_orbitals: attach Hubbard orbitals Phi ((n_orb, n_pw) complex, a row per orbital) whose
+        operator Φ V Φ' every H apply then carries with the nonlocal term; None removes them.  V starts at zero."""
+        self.n_orb = 0 if Phi is None else int(Phi.shape[0])
+        self._orb_V = None
+        check(self.ctx.L.dftk_b200_kblock_set_orbitals(self.h, self.n_orb, _ptr(Phi)), self.ctx.h)
+
+    def fold_size(self):
+        """dftk_b200_kblock_fold_size: |H| of the time-reversal fold the projector products take, 0 for complex products."""
+        n = c_i64()
+        check(self.ctx.L.dftk_b200_kblock_fold_size(self.h, ctypes.byref(n)), self.ctx.h)
+        return n.value
+
+    def set_orbital_coefficients(self, V):
+        """dftk_b200_kblock_set_orbital_coefficients: the n_orb × n_orb Hermitian orbital block of D (None = zero).
+        Re-installing the array the block already holds is free."""
+        if V is getattr(self, "_orb_V", False):
+            return
+        Vc = None if V is None else np.asfortranarray(V, dtype=np.complex128)
+        check(self.ctx.L.dftk_b200_kblock_set_orbital_coefficients(self.h, _ptr(Vc)), self.ctx.h)
+        self._orb_V = V
 
     def apply_h(self, psi, out=None):
         out = self._new(psi.shape[0]) if out is None else out

@@ -207,6 +207,10 @@ def compute_forces(basis_or_scfres, psi=None, occupation=None, *, rho=None, per_
     else:
         basis = basis_or_scfres
     model = basis.model
+    if "Hubbard" in model.term_names:
+        # the ortho-atomic orbitals depend on every position through S^{-1/2}: no Hubbard force is implemented, and
+        # leaving the term out would return forces of a different energy
+        raise NotImplementedError("compute_forces: forces of a model with a Hubbard term are not implemented")
     parts = {}
     for name in model.term_types:
         if name == "AtomicLocal":

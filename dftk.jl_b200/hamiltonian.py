@@ -23,12 +23,15 @@ class DftHamiltonianBlock:
         ops = [o for o in operators if not isinstance(o, NoopOperator)]
         fourier = [o for o in ops if isinstance(o, FourierMultiplication)]
         real = [o for o in ops if isinstance(o, RealSpaceMultiplication)]
-        nonloc = [o for o in ops if isinstance(o, NonlocalOperator)]
-        if len(fourier) > 1 or len(nonloc) > 1 or len(fourier) + len(real) + len(nonloc) != len(ops):
+        nonloc = [o for o in ops if isinstance(o, NonlocalOperator) and not o.hubbard]
+        hub = [o for o in ops if isinstance(o, NonlocalOperator) and o.hubbard]
+        if (len(fourier) > 1 or len(nonloc) > 1 or len(hub) > 1
+                or len(fourier) + len(real) + len(nonloc) + len(hub) != len(ops)):
             raise NotImplementedError("only DFT Hamiltonians (one Fourier multiplication, local potentials, "
-                                      "at most one nonlocal operator) are supported by this GPU back end")
+                                      "at most one atomic and one Hubbard nonlocal operator) are supported by this GPU back end")
         self.fourier_op = fourier[0] if fourier else None
         self.nonlocal_op = nonloc[0] if nonloc else None
+        self.hubbard_op = hub[0] if hub else None
         # optimize_operators (operators.jl:213-222): sum all real-space multiplications
         self.local_op = None
         if real:
@@ -56,6 +59,9 @@ class DftHamiltonianBlock:
             # all blocks of a spin channel share the summed potential: one device copy per (grid, spin)
             self.kblock.grid.set_potential(self.kpoint.spin, self.local_op.potential)
             self.kblock.use_grid_potential(self.kpoint.spin)
+        if getattr(self.kblock, "n_orb", 0):
+            # the orbital block of D travels with the Hamiltonian too (a Noop Hubbard term is V = 0)
+            self.kblock.set_orbital_coefficients(None if self.hubbard_op is None else self.hubbard_op.D)
         return self.kblock
 
     @property
@@ -113,12 +119,13 @@ def _ksum_totals(basis, psi, occupation, eigenvalues, eF):
     return dict(zip(names, basis.comm_kpts.allreduce(vals, "sum")))
 
 
-def energy_hamiltonian(basis, psi, occupation, *, rho, eigenvalues=None, eF=None, **kw):
+def energy_hamiltonian(basis, psi, occupation, *, rho, eigenvalues=None, eF=None, hubbard_n=None, **kw):
     """Hamiltonian.jl:200-227: energies of every term + the per-k Hamiltonian blocks."""
     energies, per_term_ops = Energies(), []
     totals = _ksum_totals(basis, psi, occupation, eigenvalues, eF)
-    for name, term in zip(basis.model.term_types, basis.terms):
-        E, ops = term.ene_ops(basis, psi, occupation, rho=rho, eigenvalues=eigenvalues, eF=eF, ksum_total=totals.get(name))
+    for name, term in zip(basis.model.term_names, basis.terms):
+        E, ops = term.ene_ops(basis, psi, occupation, rho=rho, eigenvalues=eigenvalues, eF=eF, ksum_total=totals.get(name),
+                              hubbard_n=hubbard_n)
         energies[name] = E
         per_term_ops.append(ops)
     pot_cache = {}
@@ -127,11 +134,11 @@ def energy_hamiltonian(basis, psi, occupation, *, rho, eigenvalues=None, eF=None
     return energies, Hamiltonian(basis, blocks)
 
 
-def energy(basis, psi, occupation, *, rho, eigenvalues=None, eF=None, **kw):
+def energy(basis, psi, occupation, *, rho, eigenvalues=None, eF=None, hubbard_n=None, **kw):
     """Hamiltonian.jl:232-236 (energies only)."""
     energies = Energies()
     totals = _ksum_totals(basis, psi, occupation, eigenvalues, eF)
-    for name, term in zip(basis.model.term_types, basis.terms):
+    for name, term in zip(basis.model.term_names, basis.terms):
         energies[name] = term.ene_ops(basis, psi, occupation, rho=rho, eigenvalues=eigenvalues, eF=eF,
-                                      ksum_total=totals.get(name))[0]
+                                      ksum_total=totals.get(name), hubbard_n=hubbard_n)[0]
     return energies

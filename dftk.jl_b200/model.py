@@ -96,7 +96,8 @@ class Model:
             raise ValueError("Only :none, :collinear and :spinless allowed for spin_polarization")
         self.spin_polarization = spin_polarization
         self.n_spin_components = 2 if spin_polarization == "collinear" else 1
-        self.term_types = list(terms)
+        self.term_types = list(terms)          # names, or term objects such as Hubbard(...) (called with the basis)
+        self.term_names = [t if isinstance(t, str) else t.name for t in self.term_types]
         self.functionals = list(functionals)
         groups = {}
         for i, a in enumerate(self.atoms):
@@ -125,7 +126,7 @@ def model_atomic(lattice, atoms, positions, *, extra_terms=(), **kwargs):
     return Model(lattice, atoms, positions, terms=terms, **kwargs)
 
 
-def model_DFT(lattice, atoms, positions, *, functionals, **kwargs):
-    """standard_models.jl:116-134: atomic model + Hartree + Xc(functionals)."""
-    return model_atomic(lattice, atoms, positions, extra_terms=("Hartree", "Xc"), functionals=functionals,
+def model_DFT(lattice, atoms, positions, *, functionals, extra_terms=(), **kwargs):
+    """standard_models.jl:116-134: atomic model + Hartree + Xc(functionals) + extra_terms (e.g. Hubbard(...))."""
+    return model_atomic(lattice, atoms, positions, extra_terms=("Hartree", "Xc", *extra_terms), functionals=functionals,
                         model_name="DFT", **kwargs)

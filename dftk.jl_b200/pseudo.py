@@ -45,6 +45,12 @@ class PspHgh:
     def count_n_proj(self):
         return sum((2 * l + 1) * self.h[l].shape[0] for l in range(self.lmax + 1))
 
+    def count_n_pswfc_radial(self, l=None):
+        """NormConservingPsp.jl:236: analytic HGH pseudopotentials carry no pseudo-atomic orbitals."""
+        raise ValueError(f"Pseudopotential {self.identifier} does not implement atomic wavefunctions.")
+
+    count_n_pswfc = count_n_pswfc_radial
+
     def eval_psp_local_fourier(self, p):
         """p: torch tensor of |G| values.  PspHgh.jl:110-124."""
         t = p * self.rloc
@@ -159,7 +165,7 @@ class PspUpf:
     (dftk_b200_radial_transform), once per distinct |q| of a call."""
 
     def __init__(self, Zion, lmax, rgrid, vloc, r2_projs, h, r2_rhoion, r2_rhocore, r2_taucore, identifier="",
-                 description=""):
+                 description="", r2_pswfcs=None, pswfc_labels=None, pswfc_occs=None):
         self.Zion, self.lmax = int(Zion), int(lmax)
         self.rgrid = np.ascontiguousarray(rgrid, dtype=np.float64)
         self.vloc = np.asarray(vloc, dtype=np.float64)
@@ -170,6 +176,10 @@ class PspUpf:
         self.r2_taucore = np.asarray(r2_taucore, dtype=np.float64)     # read and kept; meta-GGA is not supported
         self.rcut = float(self.rgrid[-1])
         self.identifier, self.description = identifier, description
+        # pseudo-atomic orbitals r²χ per l <= lmax (PP_PSWFC, PspUpf.jl:140-155), with their labels and occupations
+        self.r2_pswfcs = [[np.asarray(f, dtype=np.float64) for f in fl] for fl in (r2_pswfcs or [[]] * (self.lmax + 1))]
+        self.pswfc_labels = [list(x) for x in (pswfc_labels or [[]] * (self.lmax + 1))]
+        self.pswfc_occs = [list(x) for x in (pswfc_occs or [[]] * (self.lmax + 1))]
         # default_psp_quadrature: the rule is chosen on the full mesh, (x2-x1) ≈ (x3-x2) with Julia's rtol √eps, atol 0
         r = self.rgrid
         if len(r) <= 4:
@@ -185,6 +195,30 @@ class PspUpf:
 
     def count_n_proj(self):
         return sum((2 * l + 1) * self.h[l].shape[0] for l in range(self.lmax + 1))
+
+    def count_n_pswfc_radial(self, l=None):
+        """Radial pseudo-atomic orbitals of angular momentum l, or of all l (NormConservingPsp.jl:238-240)."""
+        if l is None:
+            return sum(self.count_n_pswfc_radial(ll) for ll in range(self.lmax + 1))
+        return len(self.r2_pswfcs[l])
+
+    def count_n_pswfc(self, l=None):
+        """Orbitals including their 2l+1 angular parts (NormConservingPsp.jl:242-245)."""
+        if l is None:
+            return sum(self.count_n_pswfc(ll) for ll in range(self.lmax + 1))
+        return self.count_n_pswfc_radial(l) * (2 * l + 1)
+
+    def pswfc_label(self, i, l):
+        """Label (e.g. "3D") of the i-th (1-based) radial orbital of angular momentum l."""
+        return self.pswfc_labels[l][i - 1]
+
+    def find_pswfc(self, label):
+        """(l, i) of the orbital with this label, i 1-based (NormConservingPsp.jl:247-255)."""
+        for l in range(self.lmax + 1):
+            for i in range(1, self.count_n_pswfc_radial(l) + 1):
+                if self.pswfc_label(i, l) == label:
+                    return l, i
+        raise ValueError(f"Could not find pseudo atomic orbital with label {label} in pseudopotential {self.identifier}.")
 
     @property
     def has_core_density(self):
@@ -210,6 +244,12 @@ class PspUpf:
                         g = np.zeros(n)
                         g[:len(f)] = self.weights(len(f)) * f
                         rows.append(g)
+                        ls.append(l)
+            elif kind == "pswfc":        # the orbitals are not cut off: whole mesh, whole-mesh weights (PspUpf.jl:218-223)
+                rows, ls = [], []
+                for l in range(self.lmax + 1):
+                    for f in self.r2_pswfcs[l]:
+                        rows.append(self.weights(n) * f)
                         ls.append(l)
             elif kind == "local":        # l = 0 transform of r²(vloc + Z erf(r)/r): the smooth part of PspUpf.jl:229-242
                 rows, ls = [self.weights(n) * r * (r * self.vloc + self.Zion * _erf(r))], [0]
@@ -242,6 +282,13 @@ class PspUpf:
             self._cache = (p, self.radial_transform("proj", p))
         row = sum(self.count_n_proj_radial(ll) for ll in range(l)) + i - 1
         return self._cache[1][row]
+
+    def eval_psp_pswfc_fourier(self, i, l, p):
+        """Radial part of the i-th (1-based) orbital of angular momentum l at |q| = p, divided by p^l like the projectors;
+        one launch serves all orbitals while the caller holds on to p."""
+        if getattr(self, "_pswfc_cache", (None,))[0] is not p:
+            self._pswfc_cache = (p, self.radial_transform("pswfc", p))
+        return self._pswfc_cache[1][sum(self.count_n_pswfc_radial(ll) for ll in range(l)) + i - 1]
 
     def eval_psp_local_fourier(self, p):
         F = self.radial_transform("local", p)[0]
@@ -331,8 +378,18 @@ def parse_upf(text, identifier=""):
     r2_rhocore = rgrid ** 2 * _upf_values(nlcc)[:n] if nlcc is not None else np.zeros(n)
     tau = opt("PP_TAUMOD")
     r2_taucore = rgrid ** 2 * _upf_values(tau)[:n] if tau is not None else np.zeros(n)
+    r2_pswfcs, labels, occs = [[] for _ in range(lmax + 1)], [[] for _ in range(lmax + 1)], [[] for _ in range(lmax + 1)]
+    wfc = opt("PP_PSWFC")
+    for chi in ([c for c in wfc if c.tag.startswith("PP_CHI")] if wfc is not None else []):
+        l = int(chi.get("l"))
+        if l > lmax:
+            continue
+        r2_pswfcs[l].append(rgrid * _upf_values(chi)[:n])                   # rχ -> r²χ
+        labels[l].append((chi.get("label") or "").strip())
+        occs[l].append(float(chi.get("occupation", "0")))
     return PspUpf(round(float(hd.get("z_valence"))), lmax, rgrid, vloc, r2_projs, h, r2_rhoion, r2_rhocore, r2_taucore,
-                  identifier=identifier, description=(hd.get("comment") or "").strip())
+                  identifier=identifier, description=(hd.get("comment") or "").strip(), r2_pswfcs=r2_pswfcs,
+                  pswfc_labels=labels, pswfc_occs=occs)
 
 
 def load_psp(symbol, functional="lda"):

@@ -305,8 +305,19 @@ def next_density(ham, nbandsalg, *, eigensolver=lobpcg_hyper, psi=None, eigenval
     occ, eF, occ_g = compute_occupation(basis, eig["λ"], tol_n_elec=nbandsalg.occupation_threshold,
                                         gathered=(ev_g, w_g), return_global=True)
     names, partials = ksum_energy_partials(basis, eig["X"], occ, eig["λ"], eF)
+    hub = basis.term("Hubbard")
+    n_hub = None
+    if hub is not None:
+        # this rank's partial of the Hubbard occupation rides behind the density in the same allreduce
+        n_hub = hub.local_occupation(basis, eig["X"], occ)
+        partials = np.concatenate([partials, n_hub.real.ravel(), n_hub.imag.ravel()])
     rho, totals = compute_density(basis, eig["X"], occ, occupation_threshold=nbandsalg.occupation_threshold,
                                   packed_sums=partials)
+    if n_hub is not None:
+        tail = totals[len(names):]
+        n_hub = (tail[:n_hub.size] + 1j * tail[n_hub.size:]).reshape(n_hub.shape)
+        basis._hubbard_cache = dict(psi=eig["X"], occupation=occ, n=n_hub)
+        totals = totals[:len(names)]
     basis._ksum_cache = dict(psi=eig["X"], occupation=occ, eF=eF, totals=dict(zip(names, totals)))
     return dict(psi=eig["X"], eigenvalues=eig["λ"], occupation=occ, eF=eF, rho=rho, diagonalization=eig,
                 n_bands_converge=nconv, n_matvec=int(round(float(np.sum(stats[:, 0])))),
@@ -315,8 +326,12 @@ def next_density(ham, nbandsalg, *, eigensolver=lobpcg_hyper, psi=None, eigenval
 
 def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=None, maxiter=100,
                           mixing=None, damping=0.8, eigensolver=lobpcg_hyper, diagtolalg=None, nbandsalg=None,
-                          callback=None, compute_consistent_energies=True, seed=None, anderson_m=10):
+                          callback=None, compute_consistent_energies=True, seed=None, anderson_m=10, hubbard_n=None):
+    """self_consistent_field.jl:19-45,168-289.  `hubbard_n`: the starting Hubbard occupation of a model with a Hubbard
+    term (None: the first Hamiltonian has no Hubbard operator).  Each step's Hamiltonian uses the previous step's
+    occupation; it is recomputed from the new orbitals after every density update, never mixed, and returned."""
     model = basis.model
+    hub = basis.term("Hubbard")
     start = time.time()
     rho = guess_density(basis) if rho is None else rho
     mixing = mixing or LdosMixing()        # the reference default (self_consistent_field.jl:177); simple mixing at T = 0
@@ -328,7 +343,7 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
     gen = torch.Generator(device=basis.architecture.device)
     gen.manual_seed(int(seed if seed is not None else 0) + 7919 * basis.comm_kpts.rank)   # same `seed` on every rank
     info = dict(basis=basis, rho=rho, psi=psi, occupation=None, eigenvalues=None, eF=None, n_iter=0, n_matvec=0,
-                eigenvalues_global=None, occupation_global=None,
+                eigenvalues_global=None, occupation_global=None, hubbard_n=hubbard_n,
                 converged=False, history_Etot=[], history_drho=[], stage="iterate", algorithm="SCF")
     acc = AndersonAcceleration(m=anderson_m, ctx=basis.architecture.ctx)
 
@@ -339,7 +354,7 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
         info["n_iter"] += 1
         t0 = time.time()
         _, ham = energy_hamiltonian(basis, info["psi"], info["occupation"], rho=rho_in,
-                                    eigenvalues=info["eigenvalues"], eF=info["eF"])
+                                    eigenvalues=info["eigenvalues"], eF=info["eF"], hubbard_n=info["hubbard_n"])
         nxt = next_density(ham, nbandsalg, eigensolver=eigensolver, psi=info["psi"],
                            eigenvalues=info["eigenvalues_global"], occupation=info["occupation_global"], miniter=1,
                            tol=diagtol, generator=gen)
@@ -347,9 +362,12 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
                     eigenvalues_global=nxt["eigenvalues_global"], occupation_global=nxt["occupation_global"],
                     eF=nxt["eF"], rho_out=nxt["rho"], diagonalization=nxt["diagonalization"],
                     n_bands_converge=nxt["n_bands_converge"], n_matvec=info["n_matvec"] + nxt["n_matvec"])
+        if hub is not None:
+            from .hubbard import compute_hubbard_n
+            info["hubbard_n"] = compute_hubbard_n(hub, basis, nxt["psi"], nxt["occupation"])
         if compute_consistent_energies:
             energies = energy(basis, nxt["psi"], nxt["occupation"], rho=nxt["rho"], eigenvalues=nxt["eigenvalues"],
-                              eF=nxt["eF"])
+                              eF=nxt["eF"], hubbard_n=info["hubbard_n"])
         else:
             energies = _
         drho = nxt["rho"] - rho_in
@@ -372,8 +390,9 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
         x = acc(x, damping, fx - x)
     rho_f = info["rho_out"]
     energies, ham = energy_hamiltonian(basis, info["psi"], info["occupation"], rho=rho_f,
-                                       eigenvalues=info["eigenvalues"], eF=info["eF"])
+                                       eigenvalues=info["eigenvalues"], eF=info["eF"], hubbard_n=info["hubbard_n"])
     return dict(ham=ham, basis=basis, energies=energies, converged=info["converged"], rho=rho_f,
+                hubbard_n=info["hubbard_n"],
                 eigenvalues=info["eigenvalues"], occupation=info["occupation"], eF=info["eF"], psi=info["psi"],
                 eigenvalues_global=info["eigenvalues_global"], occupation_global=info["occupation_global"],
                 n_iter=info["n_iter"], n_matvec=info["n_matvec"], history_Etot=info["history_Etot"],

@@ -38,8 +38,10 @@ class FourierMultiplication(RealFourierOperator):
 
 
 class NonlocalOperator(RealFourierOperator):
-    def __init__(self, basis, kpoint, P, D):
-        self.basis, self.kpoint, self.P, self.D = basis, kpoint, P, D
+    """`hubbard`: the operator Φ V Φ' of TermHubbard, whose columns the k-block carries beside the atomic projectors."""
+
+    def __init__(self, basis, kpoint, P, D, hubbard=False):
+        self.basis, self.kpoint, self.P, self.D, self.hubbard = basis, kpoint, P, D, hubbard
 
 
 # ------------------------------------------------------------------ terms
@@ -421,14 +423,16 @@ _TERMS = dict(Kinetic=TermKinetic, AtomicLocal=TermAtomicLocal, AtomicNonlocal=T
 
 
 def instantiate(name, basis):
+    if not isinstance(name, str):          # a term object such as Hubbard(...): called with the basis (hubbard.jl:119)
+        return name(basis)
     if name not in _TERMS:
         raise NotImplementedError(f"term {name} is outside the hot-path scope of dftk_b200")
     return _TERMS[name](basis)
 
 
 def build_kblocks(basis):
-    """One device k-block per (k, spin): kin from Kinetic, P/D from AtomicNonlocal."""
-    kin_t, nl_t = basis.term("Kinetic"), basis.term("AtomicNonlocal")
+    """One device k-block per (k, spin): kin from Kinetic, P/D from AtomicNonlocal, the orbital columns from Hubbard."""
+    kin_t, nl_t, hub_t = basis.term("Kinetic"), basis.term("AtomicNonlocal"), basis.term("Hubbard")
     out = []
     for ik, kpt in enumerate(basis.kpoints):
         kin = kin_t.kinetic_energies[ik] if kin_t is not None else None
@@ -437,6 +441,8 @@ def build_kblocks(basis):
             P, D = nl_t.ops[ik].P, nl_t.ops[ik].D
         out.append(KBlock(basis.fft_grid, kpt.mapping.cpu().numpy(), kin=kin, P=P, D=D, spin=kpt.spin,
                           kweight=basis.kweights[ik]))
+        if hub_t is not None:
+            out[-1].set_orbitals(hub_t.P_vec[ik])
     return out
 
 

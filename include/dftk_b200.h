@@ -90,6 +90,28 @@ int dftk_b200_kblock_create(dftk_b200_grid* grid, int64_t n_pw, const int64_t* m
                             const double* kin, int64_t n_proj, const void* P, const double* D,
                             int spin, double kweight, dftk_b200_kblock** out);
 int dftk_b200_kblock_destroy(dftk_b200_kblock* kb);
+
+/* ---- DFT+U orbitals (the NonlocalOperator(Φ_k, D[σ]) of TermHubbard, src/terms/hubbard.jl:103-184) ----
+ * Attaches n_orb Hubbard orbital columns Phi (n_pw × n_orb complex, column-major, host or device) to the block: every H
+ * apply then carries [P | Φ] with D = [D 0; 0 V] in ONE pair of projector products, on every path (complex and folded
+ * DMMA products, batched small path while n_proj + n_orb <= 96, INT8 planes of gemm_backend 4).  V starts at zero.
+ * n_orb = 0 removes the orbitals.  n_proj, the nonlocal band energies and dftk_b200_nonlocal_force_rows keep covering
+ * the atomic projectors only.  The slab solver (dftk_b200_lobpcg_slab) rejects blocks with orbitals. */
+int dftk_b200_kblock_set_orbitals(dftk_b200_kblock* kb, int64_t n_orb, const void* Phi /*n_pw×n_orb*/);
+/* Plane waves of one ±q pair on which the block's projector products run when they take the time-reversal fold (Γ and
+ * other k with 2k in the reciprocal lattice, and a table with P(-q) = conj P(q), orbital columns included); 0 when the
+ * block runs the complex products. */
+int dftk_b200_kblock_fold_size(dftk_b200_kblock* kb, int64_t* n_half);
+/* Installs the orbital block V (n_orb × n_orb complex Hermitian, column-major, host or device; NULL = zero) of the
+ * block's D and refreshes the derived tables on the device.  Called every SCF step; Φ is not re-uploaded. */
+int dftk_b200_kblock_set_orbital_coefficients(dftk_b200_kblock* kb, const void* V /*n_orb×n_orb*/);
+/* Occupation matrices of the orbitals (hubbard.jl:201-232 before its mpi_sum), all k-blocks of a rank in one call:
+ * n_out[σ] += Σ_{blocks of spin σ} Σ_n w_n (Φ'ψ_n)(Φ'ψ_n)'.  psi[i]: n_pw × n_bands[i] device orbitals; occ_w_host:
+ * n_blocks × ld_w band weights (k-weight × occupation / filled occupation); n_out: n_spin × n_orb × n_orb complex
+ * column-major device array, accumulated.  Every block must carry the same n_orb.  Blocks of <= 32 bands and <= 96
+ * orbitals share one batched projection launch; one synchronisation in all. */
+int dftk_b200_orbital_occupation_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* psi,
+                                       const double* occ_w_host, int64_t ld_w, const int32_t* n_bands, void* n_out);
 /* total local potential on the real-space grid for this block's spin (sum of all
  * RealSpaceMultiplication operators, src/terms/operators.jl:213-222); N_fft doubles.  NULL = none */
 int dftk_b200_kblock_set_potential(dftk_b200_kblock* kb, const double* V);
