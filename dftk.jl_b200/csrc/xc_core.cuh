@@ -79,6 +79,8 @@ HD Dual<NV> dchain(const Dual<NV>& a, double fv, double g) {   // f(a) with f(a.
 }
 template <int NV> HD Dual<NV> dlog(const Dual<NV>& a) { return dchain(a, log(a.v), 1.0 / a.v); }
 template <int NV> HD Dual<NV> dexp(const Dual<NV>& a) { double e = exp(a.v); return dchain(a, e, e); }
+template <int NV> HD Dual<NV> dlog1p(const Dual<NV>& a) { return dchain(a, log1p(a.v), 1.0 / (1.0 + a.v)); }
+template <int NV> HD Dual<NV> dexpm1(const Dual<NV>& a) { return dchain(a, expm1(a.v), exp(a.v)); }
 template <int NV> HD Dual<NV> dsqrt(const Dual<NV>& a) { double q = sqrt(a.v); return dchain(a, q, 0.5 / q); }
 template <int NV> HD Dual<NV> datan(const Dual<NV>& a) { return dchain(a, atan(a.v), 1.0 / (1.0 + a.v * a.v)); }
 template <int NV> HD Dual<NV> dcbrt(const Dual<NV>& a) { double c = cbrt(a.v); return dchain(a, c, c / (3.0 * a.v)); }
@@ -89,11 +91,36 @@ template <int NV> HD Dual<NV> dpow(const Dual<NV>& a, double p) { return dchain(
 #define XC_LDA_C_PW 4
 #define XC_GGA_X_PBE 8
 #define XC_GGA_C_PBE 16
+// Edge semantics of libxc (restated from its documented behaviour; the values are not checked against libxc's
+// sources in this tree):
+//   XC_DENS_THRESHOLD       a point whose total density is at or below it gives zero energy and potentials;
+//   XC_DENS_THRESHOLD_SPIN  a spin channel at or below it contributes nothing to spin-resolved exchange (value and
+//                           derivatives), so a fully polarised point has finite minority potentials;
+//   XC_ZETA_THRESHOLD       (1 +- zeta)^p at or below it is frozen at the threshold with zero derivative (DBL_EPSILON);
+//   XC_SIGMA_FLOOR          sigma_uu, sigma_dd (and the unpolarised sigma) are raised to it before evaluation, the
+//                           derivatives taken at the raised value: (threshold^(4/3))^2 of the 1e-15 density threshold.
+// A negative spin density (round-off, or the extrapolation of a density mixer next to an empty channel) is raised to
+// zero before zeta is formed, the derivatives taken there, so |zeta| <= 1 always: left alone, zeta^4 and (1 + zeta)^p
+// would be extrapolated without bound (an H-atom LDA SCF diverged this way, to eigenvalues of -2e8 Ha).  libxc is
+// recalled to raise each spin density to the functional's density threshold instead (1e-12 for gga_c_pbe), which at
+// rho_dn = 0 leaves phi'(zeta) evaluated at 1 - zeta = 2 threshold / n, tens of Ha in vrho_dn at n = 0.1; that floor is
+// not adopted here and, like the values above, is not checked against libxc's sources.
 #define XC_DENS_THRESHOLD 1e-15
+#define XC_DENS_THRESHOLD_SPIN 1e-15
+#define XC_ZETA_THRESHOLD 2.220446049250313e-16
+#define XC_SIGMA_FLOOR 1e-40
 
 #define XC_PI 3.14159265358979323846
-template <class T> HD T xc_fzeta(const T& z) {
-  return (dpow(1.0 + z, 4.0 / 3.0) + dpow(1.0 - z, 4.0 / 3.0) - 2.0) / (2.5198420997897464 - 2.0);   // 2^(4/3) - 2
+// (1 + zeta)^p given opz = 1 + zeta, frozen below the zeta threshold
+template <class T> HD T xc_opz_pow(const T& opz, double p) {
+  if (opz.v <= XC_ZETA_THRESHOLD) return dchain(opz, pow(XC_ZETA_THRESHOLD, p), 0.0);
+  return dpow(opz, p);
+}
+// Spin variables of a polarised point: zeta and 1 +- zeta, the latter formed as 2 rho_s / n so that they keep
+// their relative precision as zeta -> +-1.
+template <class T> struct XcSpin { T z, opz, omz; };
+template <class T> HD T xc_fzeta(const XcSpin<T>& sp) {
+  return (xc_opz_pow(sp.opz, 4.0 / 3.0) + xc_opz_pow(sp.omz, 4.0 / 3.0) - 2.0) / (2.5198420997897464 - 2.0);   // 2^(4/3) - 2
 }
 template <class T> HD T xc_ex_unif(const T& n) { return (-0.75 * 0.98474502184269641) * n * dcbrt(n); }   // (3/pi)^(1/3)
 
@@ -107,14 +134,14 @@ HD T xc_vwn_piece(const T& x, double A, double b, double c, double x0) {
               (b * x0 / X0) * (dlog((x - x0) * (x - x0) / X) + (2.0 * (b + 2.0 * x0) / Q) * at));
 }
 template <class T>
-HD T xc_ec_vwn(const T& rs, const T* zeta) {
+HD T xc_ec_vwn(const T& rs, const XcSpin<T>* sp) {
   T x = dsqrt(rs);
   T p0 = xc_vwn_piece(x, 0.0310907, 3.72744, 12.9352, -0.10498);
-  if (!zeta) return p0;
+  if (!sp) return p0;
   T p1 = xc_vwn_piece(x, 0.01554535, 7.06042, 18.0578, -0.32500);
   T p2 = xc_vwn_piece(x, -1.0 / (6.0 * XC_PI * XC_PI), 1.13107, 13.0045, -0.0047584);
-  T fz = xc_fzeta(*zeta);
-  T z2 = (*zeta) * (*zeta);
+  T fz = xc_fzeta(*sp);
+  T z2 = sp->z * sp->z;
   T z4 = z2 * z2;
   const double fpp0 = 4.0 / (9.0 * (1.2599210498948732 - 1.0));   // 4 / (9 (2^(1/3) - 1))
   return p0 + p2 * fz * (1.0 - z4) / fpp0 + (p1 - p0) * fz * z4;
@@ -123,18 +150,18 @@ template <class T>
 HD T xc_pw_G(const T& rs, double a, double a1, double b1, double b2, double b3, double b4) {
   T s = dsqrt(rs);
   T den = (2.0 * a) * (b1 * s + b2 * rs + b3 * rs * s + b4 * rs * rs);
-  return (-2.0 * a) * (1.0 + a1 * rs) * dlog(1.0 + 1.0 / den);
+  return (-2.0 * a) * (1.0 + a1 * rs) * dlog1p(1.0 / den);   // log1p: 1 / den -> 0 at large rs
 }
 template <class T>
-HD T xc_ec_pw(const T& rs, const T* zeta, bool mod) {
+HD T xc_ec_pw(const T& rs, const XcSpin<T>* sp, bool mod) {
   const double a0 = mod ? 0.0310906908696548950 : 0.0310907, a1 = mod ? 0.01554534543482744750 : 0.01554535,
                a2 = mod ? 0.0168868639404617 : 0.0168869, fz20 = mod ? 1.709920934161365617563962776245 : 1.709921;
   T g0 = xc_pw_G(rs, a0, 0.21370, 7.5957, 3.5876, 1.6382, 0.49294);
-  if (!zeta) return g0;
+  if (!sp) return g0;
   T g1 = xc_pw_G(rs, a1, 0.20548, 14.1189, 6.1977, 3.3662, 0.62517);
   T mac = xc_pw_G(rs, a2, 0.11125, 10.357, 3.6231, 0.88026, 0.49671);
-  T fz = xc_fzeta(*zeta);
-  T z2 = (*zeta) * (*zeta);
+  T fz = xc_fzeta(*sp);
+  T z2 = sp->z * sp->z;
   T z4 = z2 * z2;
   return g0 - mac * fz * (1.0 - z4) / fz20 + (g1 - g0) * fz * z4;
 }
@@ -148,20 +175,20 @@ HD T xc_ex_pbe(const T& n, const T& sigma) {
   return xc_ex_unif(n) * ((1.0 + XC_KAPPA) - XC_KAPPA / (1.0 + (mu / XC_KAPPA) * s2));
 }
 template <class T>
-HD T xc_ec_pbe(const T& n, const T& rs, const T* zeta, const T& sigma) {
+HD T xc_ec_pbe(const T& n, const T& rs, const XcSpin<T>* sp, const T& sigma) {
   const double gamma = (1.0 - 0.69314718055994531) / (XC_PI * XC_PI);
-  T ec = xc_ec_pw(rs, zeta, true);
+  T ec = xc_ec_pw(rs, sp, true);
   T phi2 = ec * 0.0 + 1.0, phi3 = ec * 0.0 + 1.0;
-  if (zeta) {
-    T phi = (dpow(1.0 + *zeta, 2.0 / 3.0) + dpow(1.0 - *zeta, 2.0 / 3.0)) * 0.5;
+  if (sp) {
+    T phi = (xc_opz_pow(sp->opz, 2.0 / 3.0) + xc_opz_pow(sp->omz, 2.0 / 3.0)) * 0.5;
     phi2 = phi * phi;
     phi3 = phi2 * phi;
   }
   T kF = dcbrt((3.0 * XC_PI * XC_PI) * n);
   T t2 = sigma / (4.0 * phi2 * ((4.0 / XC_PI) * kF) * n * n);
-  T Aa = (XC_BETA / gamma) / (dexp(-ec / (gamma * phi3)) - 1.0);
+  T Aa = (XC_BETA / gamma) / dexpm1(-ec / (gamma * phi3));
   T At2 = Aa * t2;
-  return ec + gamma * phi3 * dlog(1.0 + (XC_BETA / gamma) * t2 * (1.0 + At2) / (1.0 + At2 + At2 * At2));
+  return ec + gamma * phi3 * dlog1p((XC_BETA / gamma) * t2 * (1.0 + At2) / (1.0 + At2 + At2 * At2));
 }
 
 // One grid point.  rho: n_spin values; sigma: 1 (unpolarised) or 3 (uu, ud, dd) values, ignored for LDA.
@@ -180,44 +207,44 @@ HD void xc_point(int mask, const double* rho, const double* sigma, double* e, do
     return;
   }
   T r[NSPIN];
-  for (int s = 0; s < NSPIN; ++s) r[s] = dvar<NV>(rho[s], s);
+  for (int s = 0; s < NSPIN; ++s) {
+    r[s] = dvar<NV>(rho[s], s);
+    if (r[s].v < 0.0) r[s].v = 0.0;   // only reachable for NSPIN == 2: the total is above the threshold
+  }
   T sg[NSIG > 0 ? NSIG : 1];
-  for (int s = 0; s < NSIG; ++s) sg[s] = dvar<NV>(sigma[s], NSPIN + s);
+  for (int s = 0; s < NSIG; ++s) {
+    sg[s] = dvar<NV>(sigma[s], NSPIN + s);
+    if (s != 1 && sg[s].v < XC_SIGMA_FLOOR) sg[s].v = XC_SIGMA_FLOOR;   // sigma_ud (s == 1) is not floored
+  }
   T n = r[0];
-  T zeta = dconst<NV>(0.0);
+  XcSpin<T> sp;
   if (NSPIN == 2) {
     n = r[0] + r[1];
-    zeta = (r[0] - r[1]) / n;
-    if (zeta.v > 1.0 - 1e-14) zeta.v = 1.0 - 1e-14;
-    if (zeta.v < -1.0 + 1e-14) zeta.v = -1.0 + 1e-14;
+    sp.z = (r[0] - r[1]) / n;
+    sp.opz = 2.0 * r[0] / n;
+    sp.omz = 2.0 * r[1] / n;
   }
-  const T* zp = NSPIN == 2 ? &zeta : nullptr;
+  const XcSpin<T>* spp = NSPIN == 2 ? &sp : nullptr;
   T rs = 0.62035049089940009 / dcbrt(n);   // (3/(4 pi))^(1/3)
   T acc = dconst<NV>(0.0);
   if (mask & XC_LDA_X) {
     if (NSPIN == 1) acc = acc + xc_ex_unif(n);
     else
-      for (int s = 0; s < NSPIN; ++s) {
-        T rr = r[s];
-        if (rr.v < 1e-30) rr.v = 1e-30;
-        acc = acc + 0.5 * xc_ex_unif(2.0 * rr);
-      }
+      for (int s = 0; s < NSPIN; ++s)
+        if (r[s].v > XC_DENS_THRESHOLD_SPIN) acc = acc + 0.5 * xc_ex_unif(2.0 * r[s]);
   }
-  if (mask & XC_LDA_C_VWN) acc = acc + n * xc_ec_vwn(rs, zp);
-  if (mask & XC_LDA_C_PW) acc = acc + n * xc_ec_pw(rs, zp, false);
+  if (mask & XC_LDA_C_VWN) acc = acc + n * xc_ec_vwn(rs, spp);
+  if (mask & XC_LDA_C_PW) acc = acc + n * xc_ec_pw(rs, spp, false);
   if (GGA && (mask & XC_GGA_X_PBE)) {
     if (NSPIN == 1) acc = acc + xc_ex_pbe(n, sg[0]);
     else
-      for (int s = 0; s < NSPIN; ++s) {
-        T rr = r[s];
-        if (rr.v < 1e-30) rr.v = 1e-30;
-        acc = acc + 0.5 * xc_ex_pbe(2.0 * rr, 4.0 * sg[s == 0 ? 0 : (NSIG - 1)]);
-      }
+      for (int s = 0; s < NSPIN; ++s)
+        if (r[s].v > XC_DENS_THRESHOLD_SPIN) acc = acc + 0.5 * xc_ex_pbe(2.0 * r[s], 4.0 * sg[s == 0 ? 0 : (NSIG - 1)]);
   }
   if (GGA && (mask & XC_GGA_C_PBE)) {
     T st = sg[0];
     if (NSPIN == 2) st = sg[0] + 2.0 * sg[NSIG > 1 ? 1 : 0] + sg[NSIG > 2 ? 2 : 0];
-    acc = acc + n * xc_ec_pbe(n, rs, zp, st);
+    acc = acc + n * xc_ec_pbe(n, rs, spp, st);
   }
   *e = acc.v;
   for (int s = 0; s < NSPIN; ++s) vrho[s] = acc.d[s];

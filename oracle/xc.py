@@ -75,6 +75,8 @@ def _f1(x, f, df):
 
 def dlog(x): return _f1(x, np.log, lambda v: 1 / v)
 def dexp(x): return _f1(x, np.exp, np.exp)
+def dlog1p(x): return _f1(x, np.log1p, lambda v: 1 / (1 + v))
+def dexpm1(x): return _f1(x, np.expm1, np.exp)
 def dsqrt(x): return _f1(x, np.sqrt, lambda v: 0.5 / np.sqrt(v))
 def datan(x): return _f1(x, np.arctan, lambda v: 1 / (1 + v * v))
 def dcbrt(x): return _f1(x, np.cbrt, lambda v: np.cbrt(v) / (3 * v))
@@ -86,8 +88,30 @@ _FZ_DEN = 2 ** (4 / 3) - 2
 _FPP0 = 4 / (9 * (2 ** (1 / 3) - 1))
 
 
-def _fzeta(z):
-    return ((1 + z) ** (4 / 3) + (1 - z) ** (4 / 3) - 2) / _FZ_DEN
+# libxc's edge semantics (restated from its documented behaviour; the values are not checked against libxc's sources
+# in this tree): a point with total density at or below DENS_THRESHOLD is zero; a spin channel at or below
+# DENS_THRESHOLD_SPIN contributes nothing to spin-resolved exchange; (1 +- zeta)^p at or below ZETA_THRESHOLD
+# (DBL_EPSILON) is frozen there with zero derivative; sigma_uu, sigma_dd are raised to SIGMA_FLOOR, the square of
+# the sigma threshold 1e-15^(4/3), with derivatives taken at the raised value.  A negative spin density is raised to
+# zero before zeta is formed (derivatives taken there), so that |zeta| <= 1; libxc is recalled to raise it to the
+# density threshold instead, which is not adopted (see xc_core.cuh).
+DENS_THRESHOLD = 1e-15
+DENS_THRESHOLD_SPIN = 1e-15
+ZETA_THRESHOLD = 2.220446049250313e-16
+SIGMA_FLOOR = 1e-40
+
+
+def _opz_pow(opz, p):
+    """(1 + zeta)^p given opz = 1 + zeta, frozen below the zeta threshold."""
+    frozen = opz.v <= ZETA_THRESHOLD
+    x = np.where(frozen, 1.0, opz.v)
+    return Dual(np.where(frozen, ZETA_THRESHOLD ** p, x ** p),
+                np.where(frozen, 0.0, opz.d * (p * x ** (p - 1))))
+
+
+def _fzeta(spin):
+    _, opz, omz = spin
+    return (_opz_pow(opz, 4 / 3) + _opz_pow(omz, 4 / 3) - 2) / _FZ_DEN
 
 
 def _ex_unif_unpol(rho):
@@ -109,13 +133,13 @@ _VWN = dict(A=(0.0310907, 0.01554535, -1 / (6 * math.pi ** 2)),
             x0=(-0.10498, -0.32500, -0.0047584))
 
 
-def _ec_vwn(rs, zeta):
+def _ec_vwn(rs, spin):
     x = dsqrt(rs)
     p = [_vwn_piece(x, _VWN["A"][i], _VWN["b"][i], _VWN["c"][i], _VWN["x0"][i]) for i in range(3)]
-    if zeta is None:
+    if spin is None:
         return p[0]
-    fz = _fzeta(zeta)
-    z4 = zeta ** 4
+    fz = _fzeta(spin)
+    z4 = spin[0] ** 4
     return p[0] + p[2] * fz * (1 - z4) / _FPP0 + (p[1] - p[0]) * fz * z4
 
 
@@ -132,17 +156,17 @@ def _pw_G(rs, i, par):
     c = _PW_COMMON
     srs = dsqrt(rs)
     den = 2 * a * (c["b1"][i] * srs + c["b2"][i] * rs + c["b3"][i] * rs * srs + c["b4"][i] * rs * rs)
-    return -2 * a * (1 + c["a1"][i] * rs) * dlog(1 + 1 / den)
+    return -2 * a * (1 + c["a1"][i] * rs) * dlog1p(1 / den)
 
 
-def _ec_pw(rs, zeta, par):
+def _ec_pw(rs, spin, par):
     g0 = _pw_G(rs, 0, par)
-    if zeta is None:
+    if spin is None:
         return g0
     g1 = _pw_G(rs, 1, par)
     mac = _pw_G(rs, 2, par)  # this is -alpha_c
-    fz = _fzeta(zeta)
-    z4 = zeta ** 4
+    fz = _fzeta(spin)
+    z4 = spin[0] ** 4
     return g0 - mac * fz * (1 - z4) / par["fz20"] + (g1 - g0) * fz * z4
 
 
@@ -160,27 +184,24 @@ def _ex_pbe_unpol(rho, sigma):
     return _ex_unif_unpol(rho) * Fx
 
 
-def _ec_pbe(rho, rs, zeta, sigma_tot):
-    ec = _ec_pw(rs, zeta, _PWMOD)
-    if zeta is None:
+def _ec_pbe(rho, rs, spin, sigma_tot):
+    ec = _ec_pw(rs, spin, _PWMOD)
+    if spin is None:
         phi = 1.0
         phi3 = 1.0
     else:
-        phi = ((1 + zeta) ** (2 / 3) + (1 - zeta) ** (2 / 3)) / 2
+        phi = (_opz_pow(spin[1], 2 / 3) + _opz_pow(spin[2], 2 / 3)) / 2
         phi3 = phi * phi * phi
     kF = dcbrt(3 * math.pi ** 2 * rho)
     ks2 = 4 * kF / math.pi
     t2 = sigma_tot / (4 * (phi * phi) * ks2 * rho * rho)
-    A = (_BETA / _GAMMA) / (dexp(-ec / (_GAMMA * phi3)) - 1)
+    A = (_BETA / _GAMMA) / dexpm1(-ec / (_GAMMA * phi3))
     At2 = A * t2
-    H = _GAMMA * phi3 * dlog(1 + (_BETA / _GAMMA) * t2 * (1 + At2) / (1 + At2 + At2 * At2))
+    H = _GAMMA * phi3 * dlog1p((_BETA / _GAMMA) * t2 * (1 + At2) / (1 + At2 + At2 * At2))
     return ec + H
 
 
 # ------------------------------------------------------------------ driver
-DENS_THRESHOLD = 1e-15
-
-
 def evaluate(functionals, rho, sigma=None):
     """rho: (n_spin, N) array; sigma: None (LDA) or (n_sigma, N) with n_sigma = 1 (unpolarised)
     or 3 (uu, ud, dd).  Returns dict(e=(N,), Vrho=(n_spin,N), Vsigma=(n_sigma,N) or None), the
@@ -199,20 +220,27 @@ def evaluate(functionals, rho, sigma=None):
         d[i] = 1.0
         return Dual(val.copy(), d)
 
-    r = [var(s, safe[s]) for s in range(n_spin)]
+    r = [var(s, np.maximum(safe[s], 0.0)) for s in range(n_spin)]
     sg = None
     if is_gga:
         ssafe = np.where(mask, sigma, 0.0)
+        floored = [0] if sigma.shape[0] == 1 else [0, 2]      # sigma_ud is not floored
+        ssafe[floored] = np.maximum(ssafe[floored], SIGMA_FLOOR)
         sg = [var(n_spin + i, ssafe[i]) for i in range(sigma.shape[0])]
     if n_spin == 1:
         n = r[0]
-        zeta = None
+        spin = None
     else:
         n = r[0] + r[1]
-        zeta = (r[0] - r[1]) / n
-        # keep |zeta| < 1 for the fractional powers
-        zeta = Dual(np.clip(zeta.v, -1 + 1e-14, 1 - 1e-14), zeta.d)
+        # zeta and 1 +- zeta = 2 rho_s / n, which keep their relative precision as zeta -> +-1
+        spin = ((r[0] - r[1]) / n, 2 * r[0] / n, 2 * r[1] / n)
     rs = _RS_FAC / dcbrt(n)
+
+    def screened(s, piece):
+        """A spin channel's exchange, zero (value and derivatives) at or below the channel threshold."""
+        live = r[s].v > DENS_THRESHOLD_SPIN
+        x = piece(Dual(np.where(live, r[s].v, 1.0), r[s].d))
+        return Dual(np.where(live, x.v, 0.0), np.where(live[None, :], x.d, 0.0))
     e = Dual(np.zeros(N), np.zeros((nvar, N)))
     for f in functionals:
         if f == "lda_x":
@@ -220,22 +248,20 @@ def evaluate(functionals, rho, sigma=None):
                 e = e + _ex_unif_unpol(n)
             else:
                 for s in range(2):
-                    rs2 = Dual(np.maximum(r[s].v, 1e-30), r[s].d)
-                    e = e + 0.5 * _ex_unif_unpol(2 * rs2)
+                    e = e + screened(s, lambda rr: 0.5 * _ex_unif_unpol(2 * rr))
         elif f == "lda_c_vwn":
-            e = e + n * _ec_vwn(rs, zeta)
+            e = e + n * _ec_vwn(rs, spin)
         elif f == "lda_c_pw":
-            e = e + n * _ec_pw(rs, zeta, _PW)
+            e = e + n * _ec_pw(rs, spin, _PW)
         elif f == "gga_x_pbe":
             if n_spin == 1:
                 e = e + _ex_pbe_unpol(n, sg[0])
             else:
                 for s, isg in ((0, 0), (1, 2)):
-                    rs2 = Dual(np.maximum(r[s].v, 1e-30), r[s].d)
-                    e = e + 0.5 * _ex_pbe_unpol(2 * rs2, 4 * sg[isg])
+                    e = e + screened(s, lambda rr: 0.5 * _ex_pbe_unpol(2 * rr, 4 * sg[isg]))
         elif f == "gga_c_pbe":
             stot = sg[0] if n_spin == 1 else sg[0] + 2 * sg[1] + sg[2]
-            e = e + n * _ec_pbe(n, rs, zeta, stot)
+            e = e + n * _ec_pbe(n, rs, spin, stot)
         else:
             raise NotImplementedError(f)
     ev = np.where(mask, e.v, 0.0)
