@@ -273,8 +273,13 @@ void kb_apply_local_kinetic(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, i
       void* a1[] = {&kb->T, &twx, &p, &ld, &W1, &L, &Lp};
       launch_ptr(ctx, g->rx->sphere_to_xt, dim3(cdiv(kb->T.n_cols, L), nb), L * g->rx->T, sm_x, a1);
       const double* Vt = kb->Vtp();
-      void* a2[] = {&kb->T, &twy, &W1, &Vt};
-      launch_ptr(ctx, g->ry->yz_apply, dim3(nb, g->nx), kYzLines * g->ry->T, yz_smem(g->ny, kb->T.n_zc), a2);
+      void* a2[] = {&kb->T, &twy, &W1, &Vt, &nb};
+      // persistent: as many CTAs as are resident at once (one per SM at the larger grids), each loops over items
+      const size_t sm_yz = yz_smem(g->ny, kb->T.n_zc);
+      int per_sm = 1;
+      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, g->ry->yz_apply, g->ry->yz_threads, sm_yz));
+      const unsigned yz_ctas = (unsigned)std::min<int64_t>((int64_t)nb * g->nx, (int64_t)std::max(per_sm, 1) * ctx->sm_count);
+      launch_ptr(ctx, g->ry->yz_apply, dim3(yz_ctas), g->ry->yz_threads, sm_yz, a2);
       cplx* out = hpsi + b0 * kb->n_pw;
       double scale = 1.0;
       const double* kin = with_kin ? kb->kin.p : nullptr;

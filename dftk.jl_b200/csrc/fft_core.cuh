@@ -29,6 +29,26 @@
 #define TLOOPC(t, n, nthr) for (int t = 0; t < (n); ++t)
 #define TLOOPU(t, n) for (int t = 0; t < (n); ++t)
 #endif
+// threadIdx.x read anew at every use: what a group thread derives from its index (twiddles, plane maps) is then recomputed
+// per round instead of being hoisted out of a persistent kernel's item loop into registers for the whole kernel.
+__device__ __forceinline__ int tid_volatile() {
+  int t;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+  return t;
+}
+// Warp groups: a CTA of blockDim == G * GT threads split into G groups of GT (a multiple of 32) consecutive threads that
+// work on disjoint data between CTA-wide barriers.  GLOOP(g, G, GT) runs its body for the thread's own group g on the
+// device and for every group in turn on the host; GTLOOP(t, GT) is TLOOP over the group's threads; GSYNC(g, GT) is the
+// group's named barrier 1 + g (barrier 0 is __syncthreads).  As for TSYNC, no register state is live across a GSYNC.
+#if defined(__CUDA_ARCH__)
+#define GLOOP(g, G, GT) for (int g = (int)threadIdx.x / (GT), gonce__ = 1; gonce__; gonce__ = 0)
+#define GTLOOP(t, GT) for (int t = tid_volatile() % (GT), tonce__ = 1; tonce__; tonce__ = 0)
+#define GSYNC(g, GT) asm volatile("bar.sync %0, %1;" ::"r"(1 + (g)), "r"(GT) : "memory")
+#else
+#define GLOOP(g, G, GT) for (int g = 0; g < (G); ++g)
+#define GTLOOP(t, GT) for (int t = 0; t < (GT); ++t)
+#define GSYNC(g, GT) ((void)(g))
+#endif
 #define HD __host__ __device__ __forceinline__
 
 namespace dftk {

@@ -64,11 +64,15 @@ kr_x_to_sphere(SphereTablesX T, const cplx* tw, const cplx* W1, cplx* out, int64
   reg_x_to_sphere<A, B, XM>(T, tw, W1, out, ldout, scale, kin, psi, ldpsi, accumulate, L, Lp, (cplx*)dyn_smem_reg,
                         Dim3i{(int)blockIdx.x, (int)blockIdx.y, 0});
 }
-// fused y and z passes of the local H apply (ny == nz): one CTA per (band, x line), grid (bands, nx)
+// fused y and z passes of the local H apply (ny == nz): persistent CTAs over the items (band, x line) of nb bands, item
+// i = x * nb + band, so that the CTAs in flight share a few x lines and their Vt planes stay in L2.  No CTA barrier
+// between items: a group goes on to the next item's y backward as soon as it has finished this one's y forward.
 template <int A, int B>
-__global__ void __launch_bounds__(RegYZ<A, B>::LL * RegYZ<A, B>::T, 1)
-kr_yz_apply(SphereTablesX T, const cplx* tw, cplx* W1t, const double* Vt) {
-  reg_yz_apply<A, B>(T, tw, W1t, Vt, (cplx*)dyn_smem_reg, Dim3i{(int)blockIdx.y, 0, (int)blockIdx.x});
+__global__ void __launch_bounds__(RegYZ<A, B>::NT, 1)
+kr_yz_apply(SphereTablesX T, const cplx* tw, cplx* W1t, const double* Vt, int nb) {
+  const int n_items = nb * T.nx;
+  for (int i = blockIdx.x; i < n_items; i += gridDim.x)
+    reg_yz_apply<A, B>(T, tw, W1t, Vt, (cplx*)dyn_smem_reg, Dim3i{i / nb, 0, i % nb});
 }
 
 // ---- the same five H-apply stages for MANY k-blocks in one launch (batched small-matrix LOBPCG, lobpcg.cu): the band
@@ -134,6 +138,7 @@ static RegKernels make_entry() {
   k.A = A;
   k.B = B;
   k.T = RegPair<A, B>::T;
+  k.yz_threads = RegYZ<A, B>::NT;
   k.sphere_to_x = (const void*)kr_sphere_to_x<A, B, 0>;
   k.sphere_to_xt = (const void*)kr_sphere_to_x<A, B, 1>;
   k.y_backward = (const void*)kr_y_backward<A, B>;

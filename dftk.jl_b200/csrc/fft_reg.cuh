@@ -421,131 +421,154 @@ HD void reg_y_forward(const SphereTablesX& T, const cplx* __restrict__ tw, const
 // The y and z passes of the local H apply for one x line of one band (ny == nz, so both axes use the pair (A, B) and one
 // twiddle table).  The whole pruned y-z intermediate of the line, S[zc][y] (n_zc * (n|1) complex numbers), stays in
 // shared memory, so only the x-major W1 row W1t[band][x][0:n_cols] crosses global memory, once in and once out:
-//   y backward: the sphere columns of LL planes at a time -> S rows
-//   z apply:    LL y lines at a time: S[zc][y] -> inverse z transform -> * Vt(x, y, .) -> forward z transform -> S[zc][y]
-//   y forward:  LL S rows at a time -> the sphere columns of the plane, back into W1t in place
-// E[line][n|1] is the exchange buffer of every pass (the y passes read or write S / W1t on the other side); the two
-// exchanges of the z pass alias on the device as in reg_z_apply_potential.  Grid (bands, nx); blockDim == LL * T.
-// LL = 25 lines per round: fewer, fuller rounds hide more latency in the single CTA per SM (at 150^3 with 71 planes the
-// buffers take 231 936 of the H100's 232 448 bytes, and 150 y lines are exactly six rounds; 16 lines ran 15 % slower).
+//   y backward: the sphere columns of GL planes at a time -> S rows
+//   z apply:    GL y lines at a time: S[zc][y] -> inverse z transform -> * Vt(x, y, .) -> forward z transform -> S[zc][y]
+//   y forward:  GL S rows at a time -> the sphere columns of the plane, back into W1t in place
+// The CTA is G warp groups (GLOOP).  Group g owns a contiguous, balanced share of the planes (the same in both y passes)
+// and of the y lines (z pass), GL lines of the exchange buffer E[line][n|1] (the y passes read or write S / W1t on the
+// other side) and a named barrier, so the rounds of the groups overlap and only the two pass boundaries wait for the
+// whole CTA.  The two exchanges of the z pass alias on the device as in reg_z_apply_potential, behind the group's barrier.
+// GL = 8: the line is the fastest index of a group's threads, and 8 lines at the odd stride n|1 keep the 16-byte shared
+// accesses of every quarter warp conflict-free.  Up to G = 3 groups use 24 of the LL = 25 exchange lines of smem() (at
+// 150^3 with 71 planes the buffers take 231 936 of the H100's 232 448 bytes, one CTA per SM); fewer groups for T > 16,
+// so that a CTA has at most 12 warps and a thread may keep 168 registers.
 template <int A, int B>
 struct RegYZ {
   static constexpr int n = A * B, T = RegPair<A, B>::T, LL = 25, Sy = n | 1;   // odd row stride: conflict-free columns
+  static constexpr int GL = 8, GW = (GL * T + 31) / 32;                          // lines per round, warps per group
+  static constexpr int G = (12 / GW < 3 ? 12 / GW : 3), GT = 32 * GW, NT = G * GT;   // groups, threads per group / CTA
+  static_assert(G >= 1 && G * GL <= LL, "the groups' exchange lines must fit the buffer");
   static size_t smem(int n_zc) { return ((size_t)n_zc + (DFTK_Z_ALIAS ? 1 : 2) * LL) * Sy * sizeof(cplx); }
 };
 
+// One item (band bid.z, x line bid.x); blockDim == RegYZ<A, B>::NT.  A group touches only its own planes and exchange
+// lines after the last CTA barrier, so the device kernel may start a group on its next item without one.
 template <int A, int B>
 HD void reg_yz_apply(const SphereTablesX& T, const cplx* __restrict__ tw, cplx* __restrict__ W1t,
                      const double* __restrict__ Vt, cplx* sm, Dim3i bid) {
-  constexpr int n = A * B, TT = RegYZ<A, B>::T, LL = RegYZ<A, B>::LL, Sy = RegYZ<A, B>::Sy;
+  constexpr int n = A * B, LL = RegYZ<A, B>::LL, Sy = RegYZ<A, B>::Sy;
+  constexpr int GL = RegYZ<A, B>::GL, G = RegYZ<A, B>::G, GT = RegYZ<A, B>::GT;
   const int n_zc = T.n_zc, x = bid.x;
   cplx* S = sm;
-  cplx* E = sm + (size_t)n_zc * Sy;
-  cplx* E2 = DFTK_Z_ALIAS ? E : E + (size_t)LL * Sy;
   cplx* row = W1t + ((size_t)bid.z * T.nx + x) * T.n_cols;
   const double* vx = Vt + (size_t)x * n * n;
   const uint64_t pol_keep = l2_policy_evict_last();
-  // y backward: planes zc0 .. zc0+LL-1
-  for (int zc0 = 0; zc0 < n_zc; zc0 += LL) {
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, zc = zc0 + line;
-      if (p < B && zc < n_zc) {
-        const PlaneCols pc = plane_cols(T, zc);
-        cplx v[A];
+  // y backward: the group's planes zc0 .. zc0+GL-1
+  GLOOP(g, G, GT) {
+    cplx* E = sm + ((size_t)n_zc + g * GL) * Sy;
+    const int zc1 = (g + 1) * n_zc / G;
+    for (int zc0 = g * n_zc / G; zc0 < zc1; zc0 += GL) {
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, zc = zc0 + line;
+        if (p < B && zc < zc1) {
+          const PlaneCols pc = plane_cols(T, zc);
+          cplx v[A];
 #pragma unroll
-        for (int r = 0; r < A; ++r) {
-          int c = pc.col(p + B * r);
-          v[r] = ld_pred(row + (c < 0 ? 0 : c), c >= 0);
+          for (int r = 0; r < A; ++r) {
+            int c = pc.col(p + B * r);
+            v[r] = ld_pred(row + (c < 0 ? 0 : c), c >= 0);
+          }
+          pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
         }
-        pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
       }
-    }
-    TSYNC();
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, zc = zc0 + line;
-      if (p < A && zc < n_zc) {
-        cplx X[B];
-        pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
+      GSYNC(g, GT);
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, zc = zc0 + line;
+        if (p < A && zc < zc1) {
+          cplx X[B];
+          pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
 #pragma unroll
-        for (int d = 0; d < B; ++d) S[zc * Sy + p + A * d] = X[d];
+          for (int d = 0; d < B; ++d) S[zc * Sy + p + A * d] = X[d];
+        }
       }
+      GSYNC(g, GT);
     }
-    TSYNC();
   }
-  // z apply: y lines y0 .. y0+LL-1 (S columns)
-  for (int y0 = 0; y0 < n; y0 += LL) {
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, y = y0 + line;
-      if (p < B && y < n) {
-        cplx v[A];
+  TSYNC();
+  // z apply: the group's y lines y0 .. y0+GL-1 (S columns)
+  GLOOP(g, G, GT) {
+    cplx* E = sm + ((size_t)n_zc + g * GL) * Sy;
+    cplx* E2 = DFTK_Z_ALIAS ? E : E + (size_t)LL * Sy;
+    const int y1 = (g + 1) * n / G;
+    for (int y0 = g * n / G; y0 < y1; y0 += GL) {
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, y = y0 + line;
+        if (p < B && y < y1) {
+          cplx v[A];
 #pragma unroll
-        for (int r = 0; r < A; ++r) {
-          int zc = zc_index(T, p + B * r);
-          v[r] = zc >= 0 ? S[zc * Sy + y] : make_double2(0.0, 0.0);
+          for (int r = 0; r < A; ++r) {
+            int zc = zc_index(T, p + B * r);
+            v[r] = zc >= 0 ? S[zc * Sy + y] : make_double2(0.0, 0.0);
+          }
+          pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
         }
-        pass1_store<A, B, +1>(v, p, 0, E + line * Sy, 1, tw);
       }
-    }
-    TSYNC();
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, y = y0 + line;
-      cplx Y[B];
-      if (p < A && y < n) {
-        cplx X[B];
-        pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
+      GSYNC(g, GT);
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, y = y0 + line;
+        cplx Y[B];
+        if (p < A && y < y1) {
+          cplx X[B];
+          pass2_load<A, B, +1>(X, p, 0, E + line * Sy, 1);
 #pragma unroll
-        for (int d = 0; d < B; ++d) X[d] = cscale(X[d], ld_pred_hint(vx + y * n + p + A * d, true, pol_keep));
-        pass1_compute<B, A, -1>(X, p, tw, Y);
-      }
+          for (int d = 0; d < B; ++d) X[d] = cscale(X[d], ld_pred_hint(vx + y * n + p + A * d, true, pol_keep));
+          pass1_compute<B, A, -1>(X, p, tw, Y);
+        }
 #if DFTK_Z_ALIAS
-      __syncthreads();   // every thread of the CTA runs this body exactly once (blockDim == LL*TT)
+        GSYNC(g, GT);   // every thread of the group runs this body exactly once (GTLOOP on the device)
 #endif
-      if (p < A && y < n) {
+        if (p < A && y < y1) {
 #pragma unroll
-        for (int c = 0; c < B; ++c) E2[line * Sy + c * A + p] = Y[c];
-      }
-    }
-    TSYNC();
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, y = y0 + line;
-      if (p < B && y < n) {
-        cplx X[A];
-        pass2_load<B, A, -1>(X, p, 0, E2 + line * Sy, 1);
-#pragma unroll
-        for (int f = 0; f < A; ++f) {
-          int zc = zc_index(T, p + B * f);
-          if (zc >= 0) S[zc * Sy + y] = X[f];
+          for (int c = 0; c < B; ++c) E2[line * Sy + c * A + p] = Y[c];
         }
       }
+      GSYNC(g, GT);
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, y = y0 + line;
+        if (p < B && y < y1) {
+          cplx X[A];
+          pass2_load<B, A, -1>(X, p, 0, E2 + line * Sy, 1);
+#pragma unroll
+          for (int f = 0; f < A; ++f) {
+            int zc = zc_index(T, p + B * f);
+            if (zc >= 0) S[zc * Sy + y] = X[f];
+          }
+        }
+      }
+      GSYNC(g, GT);
     }
-    TSYNC();
   }
-  // y forward: planes zc0 .. zc0+LL-1, the sphere columns back to the W1t row
-  for (int zc0 = 0; zc0 < n_zc; zc0 += LL) {
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, zc = zc0 + line;
-      if (p < B && zc < n_zc) {
-        cplx v[A];
+  TSYNC();
+  // y forward: the group's planes zc0 .. zc0+GL-1 (the same as in y backward), the sphere columns back to the W1t row
+  GLOOP(g, G, GT) {
+    cplx* E = sm + ((size_t)n_zc + g * GL) * Sy;
+    const int zc1 = (g + 1) * n_zc / G;
+    for (int zc0 = g * n_zc / G; zc0 < zc1; zc0 += GL) {
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, zc = zc0 + line;
+        if (p < B && zc < zc1) {
+          cplx v[A];
 #pragma unroll
-        for (int r = 0; r < A; ++r) v[r] = S[zc * Sy + p + B * r];
-        pass1_store<A, B, -1>(v, p, 0, E + line * Sy, 1, tw);
-      }
-    }
-    TSYNC();
-    TLOOP(t, LL * TT) {
-      const int line = t % LL, p = t / LL, zc = zc0 + line;
-      if (p < A && zc < n_zc) {
-        const PlaneCols pc = plane_cols(T, zc);
-        cplx X[B];
-        pass2_load<A, B, -1>(X, p, 0, E + line * Sy, 1);
-#pragma unroll
-        for (int d = 0; d < B; ++d) {
-          int c = pc.col(p + A * d);
-          st_pred(row + (c < 0 ? 0 : c), X[d], c >= 0);
+          for (int r = 0; r < A; ++r) v[r] = S[zc * Sy + p + B * r];
+          pass1_store<A, B, -1>(v, p, 0, E + line * Sy, 1, tw);
         }
       }
+      GSYNC(g, GT);
+      GTLOOP(t, GT) {
+        const int line = t % GL, p = t / GL, zc = zc0 + line;
+        if (p < A && zc < zc1) {
+          const PlaneCols pc = plane_cols(T, zc);
+          cplx X[B];
+          pass2_load<A, B, -1>(X, p, 0, E + line * Sy, 1);
+#pragma unroll
+          for (int d = 0; d < B; ++d) {
+            int c = pc.col(p + A * d);
+            st_pred(row + (c < 0 ? 0 : c), X[d], c >= 0);
+          }
+        }
+      }
+      GSYNC(g, GT);
     }
-    TSYNC();
   }
 }
 

@@ -9,6 +9,7 @@ struct SphereTablesX;
 // kernel entry points of the register two-pass engine for one factor pair (fft_reg.cu)
 struct RegKernels {
   int A, B, T;
+  int yz_threads;             // blockDim of yz_apply (RegYZ<A, B>::NT)
   const void *sphere_to_x, *y_backward, *z_apply, *z_to_cube, *z_from_cube, *z_density, *y_forward, *x_to_sphere;
   const void* z_apply_pipe;   // persistent, software-pipelined form of z_apply (cp.async staged input tiles)
   const void* yz_apply;       // fused y-z stage of the local H apply on an x-major W1 (ny == nz)
