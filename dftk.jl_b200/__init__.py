@@ -60,7 +60,7 @@ from ._lib import DftkB200Error, LIB_PATH
 from .device import Context, FFTGrid, KBlock
 from .architecture import B200, CPU
 from .pseudo import PspHgh, PspUpf, ElementPsp, load_psp, parse_hgh, parse_upf
-from .model import Model, model_DFT, model_atomic, LDA, PBE, SymOp, symmetry_operations
+from .model import Model, model_DFT, model_atomic, LDA, PBE, PBEsol, SymOp, symmetry_operations
 from .parallel import KpointComm, split_evenly
 from .basis import PlaneWaveBasis, MonkhorstPack, ExplicitKpoints, Kpoint, compute_fft_size
 from .terms import guess_density

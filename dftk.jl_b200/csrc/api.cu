@@ -1,6 +1,7 @@
 // extern "C" entry points of libdftk_b200 (see include/dftk_b200.h for the contract).
 #include <mutex>
 #include "structs.cuh"
+#include "xc_core.cuh"
 
 using namespace dftk;
 
@@ -825,9 +826,9 @@ int dftk_b200_xc_evaluate(dftk_b200_ctx* ctx, int functional_mask, int n_spin, i
                           const double* sigma, double* e, double* vrho, double* vsigma) {
   API_BEGIN
   REQUIRE(ctx && rho && e && vrho && n_points >= 0, "xc_evaluate: NULL argument");
-  const bool gga = (functional_mask & (8 | 16)) != 0;
+  const bool gga = (functional_mask & XC_GGA_BITS) != 0;
   REQUIRE(!gga || (sigma && vsigma), "xc_evaluate: GGA functionals need sigma and vsigma");
-  REQUIRE((functional_mask & ~31) == 0 && functional_mask != 0, "xc_evaluate: unknown functional bits");
+  REQUIRE((functional_mask & ~XC_VALID_BITS) == 0 && functional_mask != 0, "xc_evaluate: unknown functional bits");
   REQUIRE(is_device_ptr(rho) && is_device_ptr(e) && is_device_ptr(vrho), "xc_evaluate: arrays must be device memory");
   xc_evaluate(ctx, functional_mask, n_spin, gga, n_points, rho, sigma, e, vrho, vsigma);
   API_END(ctx)

@@ -3,9 +3,9 @@
 //
 // XC: the reference evaluates libxc through Libxc.jl (src/DispatchFunctional.jl:55-56,108-128; call site
 // src/terms/xc.jl:104-113).  libxc is third-party code that is not under the DFTK.jl tree; the closed forms are
-// restated here (Dirac exchange, VWN5, PW92 / PW92-mod, PBE) with libxc's constants.  Energies per volume `e`
-// and the derivatives vrho / vsigma come from ONE expression evaluated on forward-mode dual numbers, so they are
-// mutually consistent by construction.
+// restated here (Dirac exchange, VWN5, PW92 / PW92-mod, Teter-Pade, Perdew-Zunger, and the PBE, PBEsol, revPBE and
+// RPBE GGAs) with libxc's constants.  Energies per volume `e` and the derivatives vrho / vsigma come from ONE
+// expression evaluated on forward-mode dual numbers, so they are mutually consistent by construction.
 //
 // Bodies are __host__ __device__ (host emulation in tests/hostemu).
 #pragma once
@@ -91,6 +91,15 @@ template <int NV> HD Dual<NV> dpow(const Dual<NV>& a, double p) { return dchain(
 #define XC_LDA_C_PW 4
 #define XC_GGA_X_PBE 8
 #define XC_GGA_C_PBE 16
+#define XC_LDA_XC_TETER93 32
+#define XC_LDA_C_PZ 64
+#define XC_GGA_X_PBE_SOL 128
+#define XC_GGA_C_PBE_SOL 256
+#define XC_GGA_X_PBE_R 512
+#define XC_GGA_X_RPBE 1024
+// the functionals that need the contracted gradient sigma, and every bit the kernel knows
+#define XC_GGA_BITS (XC_GGA_X_PBE | XC_GGA_C_PBE | XC_GGA_X_PBE_SOL | XC_GGA_C_PBE_SOL | XC_GGA_X_PBE_R | XC_GGA_X_RPBE)
+#define XC_VALID_BITS (XC_LDA_X | XC_LDA_C_VWN | XC_LDA_C_PW | XC_LDA_XC_TETER93 | XC_LDA_C_PZ | XC_GGA_BITS)
 // Edge semantics of libxc (restated from its documented behaviour; the values are not checked against libxc's
 // sources in this tree):
 //   XC_DENS_THRESHOLD       a point whose total density is at or below it gives zero energy and potentials;
@@ -165,17 +174,79 @@ HD T xc_ec_pw(const T& rs, const XcSpin<T>* sp, bool mod) {
   T z4 = z2 * z2;
   return g0 - mac * fz * (1.0 - z4) / fz20 + (g1 - g0) * fz * z4;
 }
-#define XC_KAPPA 0.8040
-#define XC_BETA 0.06672455060314922
+// Goedecker, Teter, Hutter, Phys. Rev. B 54, 1703 (1996): the Pade fit of exchange and correlation together,
+// e_xc per electron = -(a0 + a1 rs + a2 rs^2 + a3 rs^3) / (b1 rs + b2 rs^2 + b3 rs^3 + b4 rs^4), every coefficient
+// c + f(zeta) dc.  The constants are libxc's lda_xc_teter93 as recalled, not checked against libxc's sources; with
+// them the reference's iron LDA setup (test/iron_lda.jl) reproduces its ABINIT energy and eigenvalues.
 template <class T>
-HD T xc_ex_pbe(const T& n, const T& sigma) {
-  const double mu = XC_BETA * (XC_PI * XC_PI / 3.0);
-  T kF = dcbrt((3.0 * XC_PI * XC_PI) * n);
-  T s2 = sigma / (4.0 * kF * kF * n * n);
-  return xc_ex_unif(n) * ((1.0 + XC_KAPPA) - XC_KAPPA / (1.0 + (mu / XC_KAPPA) * s2));
+HD T xc_exc_teter(const T& rs, const XcSpin<T>* sp) {
+  const double a[4] = {0.4581652932831429, 2.217058676663745, 0.7405551735357053, 0.01968227878617998};
+  const double da[4] = {0.119086804055547, 0.6157402568883345, 0.1574201515892867, 0.003532336663397157};
+  const double b[4] = {1.0, 4.504130959426697, 1.110667363742916, 0.02359291751427506};
+  const double db[4] = {0.0, 0.2673612973836267, 0.2052004607777787, 0.004200005045691381};
+  if (!sp) return -(a[0] + rs * (a[1] + rs * (a[2] + rs * a[3]))) / (rs * (b[0] + rs * (b[1] + rs * (b[2] + rs * b[3]))));
+  T fz = xc_fzeta(*sp);
+  T num = (a[0] + da[0] * fz) + rs * ((a[1] + da[1] * fz) + rs * ((a[2] + da[2] * fz) + rs * (a[3] + da[3] * fz)));
+  T den = rs * ((b[0] + db[0] * fz) + rs * ((b[1] + db[1] * fz) + rs * ((b[2] + db[2] * fz) + rs * (b[3] + db[3] * fz))));
+  return -num / den;
+}
+// Perdew, Zunger, Phys. Rev. B 23, 5048 (1981): gamma / (1 + beta1 sqrt(rs) + beta2 rs) for rs >= 1 (libxc's
+// branch point), A ln rs + B + C rs ln rs + D rs below, in the paramagnetic and ferromagnetic limits, interpolated
+// with f(zeta).  The paper's constants.
+template <class T>
+HD T xc_pz_piece(const T& rs, double gamma, double beta1, double beta2, double A, double B, double C, double D) {
+  if (rs.v >= 1.0) return gamma / (1.0 + beta1 * dsqrt(rs) + beta2 * rs);
+  T lr = dlog(rs);
+  return A * lr + B + C * rs * lr + D * rs;
 }
 template <class T>
-HD T xc_ec_pbe(const T& n, const T& rs, const XcSpin<T>* sp, const T& sigma) {
+HD T xc_ec_pz(const T& rs, const XcSpin<T>* sp) {
+  T ep = xc_pz_piece(rs, -0.1423, 1.0529, 0.3334, 0.0311, -0.048, 0.0020, -0.0116);
+  if (!sp) return ep;
+  T ef = xc_pz_piece(rs, -0.0843, 1.3981, 0.2611, 0.01555, -0.0269, 0.0007, -0.0048);
+  return ep + xc_fzeta(*sp) * (ef - ep);
+}
+#define XC_KAPPA 0.8040
+#define XC_BETA 0.06672455060314922
+#define XC_MU_PBE (XC_BETA * (XC_PI * XC_PI / 3.0))
+// The PBE enhancement factor 1 + kappa - kappa / (1 + mu s^2 / kappa): PBE (kappa 0.804, mu_PBE), PBEsol (Perdew et
+// al., Phys. Rev. Lett. 100, 136406 (2008): mu = 10/81) and revPBE (Zhang, Yang, Phys. Rev. Lett. 80, 890 (1998):
+// kappa = 1.245).  The call sites pass literals, so each folds to its constants.
+template <class T>
+HD T xc_ex_pbe(const T& n, const T& sigma, double kappa, double mu) {
+  T kF = dcbrt((3.0 * XC_PI * XC_PI) * n);
+  T s2 = sigma / (4.0 * kF * kF * n * n);
+  return xc_ex_unif(n) * ((1.0 + kappa) - kappa / (1.0 + (mu / kappa) * s2));
+}
+// RPBE (Hammer, Hansen, Norskov, Phys. Rev. B 59, 7413 (1999)): F_x = 1 + kappa (1 - exp(-mu s^2 / kappa)).
+template <class T>
+HD T xc_ex_rpbe(const T& n, const T& sigma) {
+  T kF = dcbrt((3.0 * XC_PI * XC_PI) * n);
+  T s2 = sigma / (4.0 * kF * kF * n * n);
+  return xc_ex_unif(n) * (1.0 - XC_KAPPA * dexpm1((-XC_MU_PBE / XC_KAPPA) * s2));
+}
+// The GGA exchange of mask bit BIT, for an unpolarised density n with contracted gradient sigma.
+template <int BIT, class T>
+HD T xc_ex_gga(const T& n, const T& sigma) {
+  if (BIT == XC_GGA_X_PBE) return xc_ex_pbe(n, sigma, XC_KAPPA, XC_MU_PBE);
+  if (BIT == XC_GGA_X_PBE_SOL) return xc_ex_pbe(n, sigma, XC_KAPPA, 10.0 / 81.0);
+  if (BIT == XC_GGA_X_PBE_R) return xc_ex_pbe(n, sigma, 1.245, XC_MU_PBE);
+  return xc_ex_rpbe(n, sigma);
+}
+// acc += that exchange at a point, spin-resolved as (E[2 rho_up, 4 sigma_uu] + E[2 rho_dn, 4 sigma_dd]) / 2 with a
+// channel at or below XC_DENS_THRESHOLD_SPIN left out.  r: NSPIN densities, sg: NSIG contracted gradients.
+template <int BIT, int NSPIN, int NSIG, class T>
+HD void xc_add_ex_gga(T& acc, const T& n, const T* r, const T* sg) {
+  if (NSPIN == 1) {
+    acc = acc + xc_ex_gga<BIT>(n, sg[0]);
+    return;
+  }
+  if (r[0].v > XC_DENS_THRESHOLD_SPIN) acc = acc + 0.5 * xc_ex_gga<BIT>(2.0 * r[0], 4.0 * sg[0]);
+  if (r[NSPIN - 1].v > XC_DENS_THRESHOLD_SPIN) acc = acc + 0.5 * xc_ex_gga<BIT>(2.0 * r[NSPIN - 1], 4.0 * sg[NSIG - 1]);
+}
+// PBE correlation on PW92-mod with gradient coefficient beta: beta_PBE, or 0.046 for PBEsol.
+template <class T>
+HD T xc_ec_pbe(const T& n, const T& rs, const XcSpin<T>* sp, const T& sigma, double beta) {
   const double gamma = (1.0 - 0.69314718055994531) / (XC_PI * XC_PI);
   T ec = xc_ec_pw(rs, sp, true);
   T phi2 = ec * 0.0 + 1.0, phi3 = ec * 0.0 + 1.0;
@@ -186,9 +257,9 @@ HD T xc_ec_pbe(const T& n, const T& rs, const XcSpin<T>* sp, const T& sigma) {
   }
   T kF = dcbrt((3.0 * XC_PI * XC_PI) * n);
   T t2 = sigma / (4.0 * phi2 * ((4.0 / XC_PI) * kF) * n * n);
-  T Aa = (XC_BETA / gamma) / dexpm1(-ec / (gamma * phi3));
+  T Aa = (beta / gamma) / dexpm1(-ec / (gamma * phi3));
   T At2 = Aa * t2;
-  return ec + gamma * phi3 * dlog1p((XC_BETA / gamma) * t2 * (1.0 + At2) / (1.0 + At2 + At2 * At2));
+  return ec + gamma * phi3 * dlog1p((beta / gamma) * t2 * (1.0 + At2) / (1.0 + At2 + At2 * At2));
 }
 
 // One grid point.  rho: n_spin values; sigma: 1 (unpolarised) or 3 (uu, ud, dd) values, ignored for LDA.
@@ -235,16 +306,17 @@ HD void xc_point(int mask, const double* rho, const double* sigma, double* e, do
   }
   if (mask & XC_LDA_C_VWN) acc = acc + n * xc_ec_vwn(rs, spp);
   if (mask & XC_LDA_C_PW) acc = acc + n * xc_ec_pw(rs, spp, false);
-  if (GGA && (mask & XC_GGA_X_PBE)) {
-    if (NSPIN == 1) acc = acc + xc_ex_pbe(n, sg[0]);
-    else
-      for (int s = 0; s < NSPIN; ++s)
-        if (r[s].v > XC_DENS_THRESHOLD_SPIN) acc = acc + 0.5 * xc_ex_pbe(2.0 * r[s], 4.0 * sg[s == 0 ? 0 : (NSIG - 1)]);
-  }
-  if (GGA && (mask & XC_GGA_C_PBE)) {
+  if (mask & XC_LDA_XC_TETER93) acc = acc + n * xc_exc_teter(rs, spp);
+  if (mask & XC_LDA_C_PZ) acc = acc + n * xc_ec_pz(rs, spp);
+  if (GGA && (mask & XC_GGA_X_PBE)) xc_add_ex_gga<XC_GGA_X_PBE, NSPIN, NSIG>(acc, n, r, sg);
+  if (GGA && (mask & XC_GGA_X_PBE_SOL)) xc_add_ex_gga<XC_GGA_X_PBE_SOL, NSPIN, NSIG>(acc, n, r, sg);
+  if (GGA && (mask & XC_GGA_X_PBE_R)) xc_add_ex_gga<XC_GGA_X_PBE_R, NSPIN, NSIG>(acc, n, r, sg);
+  if (GGA && (mask & XC_GGA_X_RPBE)) xc_add_ex_gga<XC_GGA_X_RPBE, NSPIN, NSIG>(acc, n, r, sg);
+  if (GGA && (mask & (XC_GGA_C_PBE | XC_GGA_C_PBE_SOL))) {
     T st = sg[0];
     if (NSPIN == 2) st = sg[0] + 2.0 * sg[NSIG > 1 ? 1 : 0] + sg[NSIG > 2 ? 2 : 0];
-    acc = acc + n * xc_ec_pbe(n, rs, spp, st);
+    if (mask & XC_GGA_C_PBE) acc = acc + n * xc_ec_pbe(n, rs, spp, st, XC_BETA);
+    if (mask & XC_GGA_C_PBE_SOL) acc = acc + n * xc_ec_pbe(n, rs, spp, st, 0.046);
   }
   *e = acc.v;
   for (int s = 0; s < NSPIN; ++s) vrho[s] = acc.d[s];

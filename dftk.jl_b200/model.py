@@ -62,6 +62,10 @@ def PBE():
     return ["gga_x_pbe", "gga_c_pbe"]  # standard_models.jl:224
 
 
+def PBEsol():
+    return ["gga_x_pbe_sol", "gga_c_pbe_sol"]  # standard_models.jl:234
+
+
 class Model:
     def __init__(self, lattice, atoms=(), positions=(), *, model_name="custom", n_electrons=None,
                  magnetic_moments=(), terms=("Kinetic",), functionals=(), temperature=0.0, smearing=None,

@@ -1,12 +1,16 @@
 """Exchange-correlation energy densities and potentials on the device (the XC dispatch point of
 ext/DFTKCUDAExt.jl:17-25): one fused CUDA kernel per evaluation (csrc/xc_core.cuh, dual-number closed forms of
-Dirac exchange, VWN5, PW92 and PBE with libxc's constants), called through dftk_b200_xc_evaluate."""
+Dirac exchange, VWN5, PW92, Teter-Pade, Perdew-Zunger, PBE, PBEsol, revPBE and RPBE with libxc's constants), called
+through dftk_b200_xc_evaluate."""
 import torch
 
 from ._lib import check
 from .device import _ptr
 
-FUNCTIONAL_BITS = {"lda_x": 1, "lda_c_vwn": 2, "lda_c_pw": 4, "gga_x_pbe": 8, "gga_c_pbe": 16}
+# libxc symbol -> mask bit of the kernel (XC_* in csrc/xc_core.cuh)
+FUNCTIONAL_BITS = {"lda_x": 1, "lda_c_vwn": 2, "lda_c_pw": 4, "gga_x_pbe": 8, "gga_c_pbe": 16, "lda_xc_teter93": 32,
+                   "lda_c_pz": 64, "gga_x_pbe_sol": 128, "gga_c_pbe_sol": 256, "gga_x_pbe_r": 512, "gga_x_rpbe": 1024}
+GGA_BITS = sum(b for f, b in FUNCTIONAL_BITS.items() if f.startswith("gga"))
 
 
 def evaluate(ctx, functionals, rho, sigma=None):
@@ -18,7 +22,7 @@ def evaluate(ctx, functionals, rho, sigma=None):
             raise NotImplementedError(f"functional {f}")
         mask |= FUNCTIONAL_BITS[f]
     n_spin, N = rho.shape
-    is_gga = bool(mask & 24)
+    is_gga = bool(mask & GGA_BITS)
     if is_gga and sigma is None:
         raise ValueError("GGA functionals need the contracted gradient sigma")
     rho = rho.contiguous()

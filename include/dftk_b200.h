@@ -204,7 +204,8 @@ int dftk_b200_allgather(dftk_b200_ctx* ctx, const void* send /*dev*/, void* recv
 
 /* ---- SCF plumbing next to the hot path (SURVEY §8f rank 1) ----
  * Pointwise exchange-correlation (replaces the Libxc dispatch, ext/DFTKCUDAExt.jl:17-25, src/terms/xc.jl:104-113).
- * functional_mask: 1 lda_x | 2 lda_c_vwn | 4 lda_c_pw | 8 gga_x_pbe | 16 gga_c_pbe.  Arrays are component-major
+ * functional_mask: 1 lda_x | 2 lda_c_vwn | 4 lda_c_pw | 8 gga_x_pbe | 16 gga_c_pbe | 32 lda_xc_teter93 | 64 lda_c_pz |
+ * 128 gga_x_pbe_sol | 256 gga_c_pbe_sol | 512 gga_x_pbe_r | 1024 gga_x_rpbe; a gga_* bit needs sigma.  Arrays are component-major
  * device doubles: rho[n_spin][n], sigma[1|3][n] (uu, ud, dd; GGA only), e[n] (energy per volume),
  * vrho[n_spin][n], vsigma[1|3][n] -- the quantities libxc returns as zk*rho, vrho, vsigma. */
 int dftk_b200_xc_evaluate(dftk_b200_ctx* ctx, int functional_mask, int n_spin, int64_t n_points,
