@@ -75,3 +75,4 @@ from .hubbard import (OrbitalManifold, Hubbard, TermHubbard, atomic_orbital_proj
 from .scf import (self_consistent_field, next_density, AdaptiveBands, FixedBands, AdaptiveDiagtol,
                   ScfConvergenceDensity, ScfConvergenceEnergy, SimpleMixing, KerkerMixing, LdosMixing, compute_ldos,
                   AndersonAcceleration, ScfDefaultCallback)
+from .direct_minimization import direct_minimization, select_occupied_orbitals

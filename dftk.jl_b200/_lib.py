@@ -69,6 +69,12 @@ SIGNATURES = {
     "dftk_b200_tall_gram": (c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp]),
     "dftk_b200_zgemm": (c_int, [c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp,
                                 c_vp, c_i64]),
+    "dftk_b200_apply_h_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "dftk_b200_stiefel_project_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64]),
+    "dftk_b200_stiefel_retract_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64]),
+    "dftk_b200_tpa_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_vp]),
+    "dftk_b200_real_dots_multi": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "dftk_b200_axpy_dot_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_dbl, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

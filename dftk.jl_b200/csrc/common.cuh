@@ -141,6 +141,10 @@ struct dftk_b200_ctx {
                               // round)
   double lobpcg_flops = 0.0;  // FP64-equivalent GEMM flops executed by the large-path LOBPCG solves (Gram, update, Cholesky-QR, nonlocal) since reset
   int64_t batch_rounds = 0;   // scheduler rounds (= host synchronisations) of the batched solves since creation / reset
+  // direct minimisation (dm.cu): item descriptors, reduction partials and results, small matrices of all blocks
+  dftk::DevBuf<char> dm_items;
+  dftk::DevBuf<double> dm_ws, dm_out, dm_w, dm_stats;
+  dftk::DevBuf<dftk::cplx> dm_C, dm_M, dm_V;
 };
 
 namespace dftk {

@@ -1923,12 +1923,9 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
 // C (nA x nB, host, column-major) = A' B for tall column-major blocks (n_rows >> nA, nB <= SMALL_MAX_COLS): one fused launch
 // (CTA partials + last-CTA reduction, lobpcg_small.cuh).  Used by the host driver for the history dot products of Anderson
 // mixing (src/scf/anderson.jl:81-130) instead of a QR factorisation of the N_fft x m history matrix.
-void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
-               cplx* out_host) {
-  REQUIRE(nA >= 1 && nB >= 1 && nA <= SMALL_MAX_COLS && nB <= SMALL_MAX_COLS, "tall_gram: 1 <= columns <= 96");
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < 256) exec.reset_counters(256);
-  cplx* C = (cplx*)ctx->batch_gather.p;       // >= 96 x 96 complex fit the gather buffer
+// One Gram item C = A' B of single tall blocks, with the CTA geometry of the batched kernel.
+static GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB,
+                                 int64_t n_rows, cplx* C) {
   GramItem g{};
   g.A.n = g.B.n = 1;
   g.A.p[0] = A; g.A.ld[0] = lda; g.A.cols[0] = nA;
@@ -1939,9 +1936,86 @@ void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cpl
   g.upper_only = 0;
   g.C = C;
   g.ldc = nA;
-  std::vector<GramItem> v{g};
+  return g;
+}
+
+void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
+               cplx* out_host) {
+  REQUIRE(nA >= 1 && nB >= 1 && nA <= SMALL_MAX_COLS && nB <= SMALL_MAX_COLS, "tall_gram: 1 <= columns <= 96");
+  BatchExec exec(ctx);
+  if (ctx->small_counter.cap < 256) exec.reset_counters(256);
+  cplx* C = (cplx*)ctx->batch_gather.p;       // >= 96 x 96 complex fit the gather buffer
+  std::vector<GramItem> v{single_gram_item(ctx, A, lda, nA, B, ldb, nB, n_rows, C)};
   exec.gram_batch(v);
   CUDA_CHECK(cudaMemcpyAsync(out_host, C, (size_t)nA * nB * sizeof(cplx), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
+// ------------------------------------------------------------------ direct minimisation (dm.cu)
+// The batched small-matrix kernels of the scheduler, for all blocks of <= SMALL_MAX_N bands in one launch each.  Every
+// call synchronises the stream before it returns: its descriptors are staged in the executor's pinned ring.
+void dm_small_gram(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* A, const cplx* const* B, int nb,
+                   cplx* C) {
+  REQUIRE(nb <= SMALL_MAX_N, "dm_small_gram: too many bands");
+  BatchExec exec(ctx);
+  if (ctx->small_counter.cap < (size_t)std::max(n, 256)) exec.reset_counters((size_t)n);
+  std::vector<GramItem> v;
+  for (int i = 0; i < n; ++i) v.push_back(single_gram_item(ctx, A[i], kbs[i]->n_pw, nb, B[i], kbs[i]->n_pw, nb, kbs[i]->n_pw, C + (size_t)i * nb * nb));
+  exec.gram_batch(v);
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
+void dm_small_times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* Y, const cplx* M, int nb,
+                    cplx* const* out, double alpha, double beta) {
+  REQUIRE(nb <= SMALL_MAX_N, "dm_small_times: too many bands");
+  BatchExec exec(ctx);
+  std::vector<BtimesItem> v;
+  for (int i = 0; i < n; ++i) {
+    BtimesItem b{};
+    b.Y.n = 1;
+    b.Y.p[0] = Y[i]; b.Y.ld[0] = kbs[i]->n_pw; b.Y.cols[0] = nb;
+    for (int q = 1; q < 4; ++q) b.Y.start[q] = nb;
+    b.cm = M + (size_t)i * nb * nb; b.ldcm = nb; b.ncols = nb;
+    b.out = out[i]; b.ldo = kbs[i]->n_pw; b.n_rows = kbs[i]->n_pw; b.alpha = alpha; b.beta = beta;
+    v.push_back(b);
+  }
+  exec.btimes_batch(v);
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
+void dm_small_heev(dftk_b200_ctx* ctx, int n, cplx* G, int nb, double* w, cplx* V, double* stats) {
+  REQUIRE(nb <= SMALL_MAX_N, "dm_small_heev: too many bands");
+  BatchExec exec(ctx);
+  std::vector<Op> ops(n);
+  std::vector<Op*> p;
+  for (int i = 0; i < n; ++i) {
+    ops[i].type = OP_HEEV;
+    ops[i].u.heev = HeevItem{G + (size_t)i * nb * nb, nb, nb, w + (size_t)i * nb, V + (size_t)i * nb * nb, stats + 2 * i, nullptr, 0};
+    p.push_back(&ops[i]);
+  }
+  exec.launch(OP_HEEV, p);
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
+void dm_kin_dots(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* X, int nb, double* out) {
+  BatchExec exec(ctx);
+  std::vector<KinDotsItem> v;
+  for (int i = 0; i < n; ++i) v.push_back(KinDotsItem{X[i], kbs[i]->n_pw, kbs[i]->n_pw, nb, kbs[i]->kin.p, out + (size_t)i * nb});
+  LAUNCH(ctx, kb_kin_dots, dim3((unsigned)nb, (unsigned)n), 256, 0, exec.upload(v));
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+}
+
+void dm_apply_h(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* in, cplx* const* out, int nb) {
+  BatchExec exec(ctx);
+  if (ctx->small_counter.cap < (size_t)std::max(n, 256)) exec.reset_counters((size_t)n);
+  std::vector<Op> ops(n);
+  std::vector<Op*> p;
+  for (int i = 0; i < n; ++i) {
+    ops[i].type = OP_APPLYH;
+    ops[i].u.applyh = ApplyHItem{kbs[i], in[i], out[i], nb};
+    p.push_back(&ops[i]);
+  }
+  exec.launch(OP_APPLYH, p);
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
 }
 

@@ -206,4 +206,13 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
 void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
                cplx* out_host);
 void lobpcg_set_attributes();
+// direct minimisation (dm.cu): the scheduler's batched small-matrix kernels on blocks of <= SMALL_MAX_N bands, all blocks at
+// once (C_i, M_i, G_i: nb x nb at offset i nb^2); dm_kin_dots and dm_apply_h take any band count
+void dm_small_gram(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* A, const cplx* const* B, int nb,
+                   cplx* C);                                                       // C_i = A_i^H B_i
+void dm_small_times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* Y, const cplx* M, int nb,
+                    cplx* const* out, double alpha, double beta);                  // out_i = alpha Y_i M_i + beta out_i
+void dm_small_heev(dftk_b200_ctx* ctx, int n, cplx* G, int nb, double* w, cplx* V, double* stats);   // eigenvectors -> G_i
+void dm_kin_dots(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* X, int nb, double* out);
+void dm_apply_h(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* in, cplx* const* out, int nb);
 }  // namespace dftk

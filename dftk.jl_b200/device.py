@@ -209,6 +209,82 @@ def random_orbitals_multi(kblocks, n_bands, seed):
     return Xs
 
 
+def _blocks(kblocks, *lists):
+    """ctypes arrays of the k-block handles and of the data pointers of each list of (n_bands, n_pw_i) tensors (None: NULL)."""
+    n = len(kblocks)
+    out = [(c_vp * n)(*[kb.h.value for kb in kblocks])]
+    for ts in lists:
+        if ts is None:
+            out.append(None)
+            continue
+        assert all(t.is_contiguous() for t in ts)
+        out.append((c_vp * len(ts))(*[t.data_ptr() for t in ts]))
+    return out
+
+
+def apply_h_multi(kblocks, psis, outs, scale=None):
+    """dftk_b200_apply_h_multi: outs[i] = scale[i] H_i psis[i] for all blocks (potentials already installed)."""
+    if not kblocks:
+        return outs
+    kb, x, o = _blocks(kblocks, psis, outs)
+    sc = None if scale is None else np.ascontiguousarray(scale, dtype=np.float64)
+    check(kblocks[0].ctx.L.dftk_b200_apply_h_multi(len(kblocks), kb, x, o, psis[0].shape[0], _ptr(sc)), kblocks[0].ctx.h)
+    return outs
+
+
+def stiefel_project_multi(kblocks, X, G):
+    """dftk_b200_stiefel_project_multi: G[i] -= X[i] herm(X[i]' G[i]) in place."""
+    if kblocks:
+        kb, x, g = _blocks(kblocks, X, G)
+        check(kblocks[0].ctx.L.dftk_b200_stiefel_project_multi(len(kblocks), kb, x, g, X[0].shape[0]), kblocks[0].ctx.h)
+    return G
+
+
+def stiefel_retract_multi(kblocks, Y):
+    """dftk_b200_stiefel_retract_multi: new tensors Y[i] (Y[i]' Y[i])^{-1/2}."""
+    out = [torch.empty_like(y) for y in Y]
+    if kblocks:
+        kb, y, o = _blocks(kblocks, Y, out)
+        check(kblocks[0].ctx.L.dftk_b200_stiefel_retract_multi(len(kblocks), kb, y, o, Y[0].shape[0]), kblocks[0].ctx.h)
+    return out
+
+
+def tpa_multi(kblocks, mean_kin, inv_w, use_tpa, X=None, Q=None, S=None):
+    """dftk_b200_tpa_multi: X given -> mean_kin (n_blocks, n_bands device tensor) from X; Q given -> S = P \\ Q."""
+    if not kblocks:
+        return S
+    nb = (X if X is not None else Q)[0].shape[0]
+    kb, x, q, s = _blocks(kblocks, X, Q, S)
+    w = np.ascontiguousarray(inv_w, dtype=np.float64)
+    check(kblocks[0].ctx.L.dftk_b200_tpa_multi(len(kblocks), kb, x, q, s, nb, _ptr(w), int(bool(use_tpa)),
+                                               _ptr(mean_kin) if use_tpa else None), kblocks[0].ctx.h)
+    return S
+
+
+def real_dots_multi(kblocks, pairs):
+    """dftk_b200_real_dots_multi: [Σ_i Re<A[i], B[i]> for (A, B) in pairs] in one reduction and one synchronisation."""
+    n = len(kblocks)
+    if n == 0:
+        return [0.0] * len(pairs)
+    A = [a for p in pairs for a in p[0]]
+    B = [b for p in pairs for b in p[1]]
+    kb, a, b = _blocks(kblocks, A, B)
+    out = np.zeros(len(pairs))
+    check(kblocks[0].ctx.L.dftk_b200_real_dots_multi(len(pairs), n, kb, a, b, A[0].shape[0], _ptr(out)), kblocks[0].ctx.h)
+    return out.tolist()
+
+
+def axpy_dot_multi(kblocks, Y, X, c, Z=None):
+    """dftk_b200_axpy_dot_multi: Y[i] += c X[i] in place, then Σ_i Re<Z[i], Y[i]> (None when Z is None)."""
+    if not kblocks:
+        return None if Z is None else 0.0
+    kb, y, x, z = _blocks(kblocks, Y, X, Z)
+    out = ctypes.c_double(0.0)
+    check(kblocks[0].ctx.L.dftk_b200_axpy_dot_multi(len(kblocks), kb, y, x, float(c), z, Y[0].shape[0], ctypes.byref(out)),
+          kblocks[0].ctx.h)
+    return None if Z is None else out.value
+
+
 class FFTGrid:
     """dftk_b200_grid (FFTGrid of src/fft.jl:57-98)."""
 

@@ -270,6 +270,33 @@ int dftk_b200_zgemm(dftk_b200_ctx* ctx, int transA, int64_t m, int64_t n, int64_
                     const double* alpha2, const void* A, int64_t lda, const void* B, int64_t ldb,
                     const double* beta2, void* C, int64_t ldc);
 
+/* ---- direct minimisation of the Kohn-Sham energy (src/scf/direct_minimization.jl).  Every call works on all listed
+ * (k, spin) blocks of one context at once; block i holds n_bands orbitals of its k-block (n_pw_i x n_bands, column-major,
+ * device).  Blocks of <= 32 bands take a fixed number of launches whatever their count.  Reductions are deterministic
+ * (fixed-order two-stage sums, no floating-point atomics): identical inputs give bit-identical results. */
+/* out[i] = scale[i] * H_i psi[i] (scale_host NULL: no scaling).  The scale is a separate elementwise pass over the outputs
+ * after the H apply (one launch for all blocks), not folded into the H apply's own output write. */
+int dftk_b200_apply_h_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* psi, void* const* out,
+                            int64_t n_bands, const double* scale_host);
+/* tangent projection onto the Stiefel manifold at X: G[i] -= X[i] (X[i]' G[i] + G[i]' X[i]) / 2 */
+int dftk_b200_stiefel_project_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* X, void* const* G,
+                                    int64_t n_bands);
+/* polar retraction: X_out[i] = Y[i] (Y[i]' Y[i])^{-1/2}, from the eigendecomposition of the Gram matrix; X_out must not alias Y.
+ * Returns DFTK_B200_ENUM when an eigensolve does not converge or a Gram matrix is not positive definite. */
+int dftk_b200_stiefel_retract_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* Y, void* const* X_out,
+                                    int64_t n_bands);
+/* TPA preconditioner of the minimiser.  X non-NULL (precondprep!): mean_kin[i * n_bands + n] = sum_G kin_G |X[i]_Gn|^2.
+ * Q non-NULL (ldiv!): S[i]_Gn = mean_kin[n] / (mean_kin[n] + kin_G) * Q[i]_Gn * inv_w[i].  use_tpa = 0: the identity,
+ * S = Q * inv_w.  mean_kin: device, n_blocks x n_bands. */
+int dftk_b200_tpa_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* X, const void* const* Q,
+                        void* const* S, int64_t n_bands, const double* inv_w_host, int use_tpa, double* mean_kin);
+/* out_host[p] = sum_i Re <A[p n_blocks + i], B[p n_blocks + i]> for p < n_pairs: two launches, one synchronisation */
+int dftk_b200_real_dots_multi(int64_t n_pairs, int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* A,
+                              const void* const* B, int64_t n_bands, double* out_host);
+/* Y[i] += c X[i], then *out_host = sum_i Re <Z[i], Y[i]> in the same pass over memory (Z NULL: the update alone) */
+int dftk_b200_axpy_dot_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, void* const* Y, const void* const* X, double c,
+                             const void* const* Z, int64_t n_bands, double* out_host);
+
 #ifdef __cplusplus
 }
 #endif
