@@ -63,10 +63,11 @@ from .pseudo import PspHgh, PspUpf, ElementPsp, load_psp, parse_hgh, parse_upf
 from .model import Model, model_DFT, model_atomic, LDA, PBE, PBEsol, SymOp, symmetry_operations
 from .parallel import KpointComm, split_evenly
 from .basis import PlaneWaveBasis, MonkhorstPack, ExplicitKpoints, Kpoint, compute_fft_size
-from .terms import guess_density
+from .terms import (guess_density, Kinetic, BlowupIdentity, BlowupCHV, BlowupAbinit, smearing_occupation,
+                    smearing_entropy, occupation_derivative)
 from .hamiltonian import Hamiltonian, DftHamiltonianBlock, energy_hamiltonian, energy, Energies
 from .eigen import lobpcg_hyper, diagonalize_all_kblocks, random_orbitals
-from .occupation import compute_occupation
+from .occupation import compute_occupation, FermiBisection, FermiTwoStage, default_fermialg
 from .densities import compute_density, symmetrize_rho
 from .forces import (compute_forces, compute_forces_cart, symmetrize_forces, energy_forces_ewald,
                      energy_forces_ewald_device)

@@ -66,6 +66,19 @@ def PBEsol():
     return ["gga_x_pbe_sol", "gga_c_pbe_sol"]  # standard_models.jl:234
 
 
+def _check_smearing(smearing):
+    """Smearing.jl: "None", "FermiDirac", "Gaussian", "MarzariVanderbilt" or ("MethfesselPaxton", order >= 0)."""
+    if isinstance(smearing, (tuple, list)) and len(smearing) == 2 and smearing[0] == "MethfesselPaxton":
+        order = smearing[1]
+        if isinstance(order, (bool, np.bool_)) or not isinstance(order, (int, np.integer)) or order < 0:
+            raise ValueError(f"Methfessel-Paxton order must be a non-negative integer, got {order!r}")
+        return ("MethfesselPaxton", int(order))
+    if isinstance(smearing, str) and smearing in ("None", "FermiDirac", "Gaussian", "MarzariVanderbilt"):
+        return smearing
+    raise NotImplementedError(f"smearing {smearing!r}: only 'None', 'FermiDirac', 'Gaussian', 'MarzariVanderbilt' and "
+                              "('MethfesselPaxton', order) are supported")
+
+
 class Model:
     def __init__(self, lattice, atoms=(), positions=(), *, model_name="custom", n_electrons=None,
                  magnetic_moments=(), terms=("Kinetic",), functionals=(), temperature=0.0, smearing=None,
@@ -87,10 +100,7 @@ class Model:
         if temperature < 0:
             raise ValueError("temperature must be non-negative")
         self.temperature = float(temperature)
-        self.smearing = smearing or ("FermiDirac" if temperature > 0 else "None")
-        if self.smearing not in ("None", "FermiDirac", "Gaussian"):
-            # the Fermi-level search of dftk_b200.occupation covers monotone smearing functions only (no FermiTwoStage)
-            raise NotImplementedError(f"smearing {self.smearing!r}: only 'None', 'FermiDirac' and 'Gaussian' are supported")
+        self.smearing = _check_smearing(smearing or ("FermiDirac" if temperature > 0 else "None"))
         self.magnetic_moments = [float(m) for m in magnetic_moments]
         if self.magnetic_moments and len(self.magnetic_moments) != len(self.atoms):
             raise ValueError("Length of atoms and magnetic_moments vectors need to agree.")
@@ -122,8 +132,11 @@ class Model:
         return 2 if self.spin_polarization == "none" else 1
 
 
-def model_atomic(lattice, atoms, positions, *, extra_terms=(), **kwargs):
-    terms = ["Kinetic", "AtomicLocal", "AtomicNonlocal", "Ewald", "PspCorrection", *extra_terms]
+def model_atomic(lattice, atoms, positions, *, extra_terms=(), kinetic_blowup=None, **kwargs):
+    """standard_models.jl:45-60; `kinetic_blowup` (BlowupCHV(), BlowupAbinit(...)) smooths the kinetic energy near Ecut."""
+    from .terms import Kinetic
+    kinetic = "Kinetic" if kinetic_blowup is None else Kinetic(blowup=kinetic_blowup)
+    terms = [kinetic, "AtomicLocal", "AtomicNonlocal", "Ewald", "PspCorrection", *extra_terms]
     if kwargs.get("temperature", 0) != 0:
         terms.append("Entropy")
     kwargs.setdefault("model_name", "atomic")

@@ -284,7 +284,7 @@ class AndersonAcceleration:
 
 
 def next_density(ham, nbandsalg, *, eigensolver=lobpcg_hyper, psi=None, eigenvalues=None, occupation=None,
-                 tol=1e-6, miniter=1, maxiter=100, generator=None):
+                 tol=1e-6, miniter=1, maxiter=100, generator=None, fermialg=None):
     """self_consistent_field.jl:80-129.  `eigenvalues` / `occupation` drive the band-count heuristics: pass the lists
     over ALL (k, spin) blocks (the `*_global` entries of the previous result) so that every rank takes the same
     decision without the mpi_max of self_consistent_field.jl:98.
@@ -302,7 +302,7 @@ def next_density(ham, nbandsalg, *, eigensolver=lobpcg_hyper, psi=None, eigenval
     if not eig["converged"]:
         import warnings
         warnings.warn(f"Eigensolver not converged, n_iter={eig['n_iter']}")
-    occ, eF, occ_g = compute_occupation(basis, eig["λ"], tol_n_elec=nbandsalg.occupation_threshold,
+    occ, eF, occ_g = compute_occupation(basis, eig["λ"], fermialg=fermialg, tol_n_elec=nbandsalg.occupation_threshold,
                                         gathered=(ev_g, w_g), return_global=True)
     names, partials = ksum_energy_partials(basis, eig["X"], occ, eig["λ"], eF)
     hub = basis.term("Hubbard")
@@ -326,10 +326,12 @@ def next_density(ham, nbandsalg, *, eigensolver=lobpcg_hyper, psi=None, eigenval
 
 def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=None, maxiter=100,
                           mixing=None, damping=0.8, eigensolver=lobpcg_hyper, diagtolalg=None, nbandsalg=None,
-                          callback=None, compute_consistent_energies=True, seed=None, anderson_m=10, hubbard_n=None):
+                          callback=None, compute_consistent_energies=True, seed=None, anderson_m=10, hubbard_n=None,
+                          fermialg=None):
     """self_consistent_field.jl:19-45,168-289.  `hubbard_n`: the starting Hubbard occupation of a model with a Hubbard
     term (None: the first Hamiltonian has no Hubbard operator).  Each step's Hamiltonian uses the previous step's
-    occupation; it is recomputed from the new orbitals after every density update, never mixed, and returned."""
+    occupation; it is recomputed from the new orbitals after every density update, never mixed, and returned.
+    `fermialg`: the Fermi-level search, FermiBisection() or FermiTwoStage() (default: default_fermialg(model.smearing))."""
     model = basis.model
     hub = basis.term("Hubbard")
     start = time.time()
@@ -357,7 +359,7 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
                                     eigenvalues=info["eigenvalues"], eF=info["eF"], hubbard_n=info["hubbard_n"])
         nxt = next_density(ham, nbandsalg, eigensolver=eigensolver, psi=info["psi"],
                            eigenvalues=info["eigenvalues_global"], occupation=info["occupation_global"], miniter=1,
-                           tol=diagtol, generator=gen)
+                           tol=diagtol, generator=gen, fermialg=fermialg)
         info.update(ham=ham, rho_in=rho_in, psi=nxt["psi"], eigenvalues=nxt["eigenvalues"], occupation=nxt["occupation"],
                     eigenvalues_global=nxt["eigenvalues_global"], occupation_global=nxt["occupation_global"],
                     eF=nxt["eF"], rho_out=nxt["rho"], diagonalization=nxt["diagonalization"],

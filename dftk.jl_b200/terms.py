@@ -9,7 +9,7 @@ work on orbitals (kinetic / nonlocal band energies) goes through libdftk_b200.
 import math
 import numpy as np
 import torch
-from scipy.special import erfc
+from scipy.special import erf, erfc
 
 from . import xc as xcmod
 from .pseudo import solid_harmonic_real, atom_decay_length
@@ -45,14 +45,90 @@ class NonlocalOperator(RealFourierOperator):
 
 
 # ------------------------------------------------------------------ terms
-class TermKinetic:
-    """kinetic.jl:14-57."""
+def _xp(p):
+    return torch if isinstance(p, torch.Tensor) else np
 
-    def __init__(self, basis, scaling_factor=1.0):
+
+class BlowupIdentity:
+    """kinetic.jl:63-67: the standard kinetic energy |p|²/2."""
+
+    def __call__(self, p, Ecut):
+        return _xp(p).ones_like(p)
+
+    def __repr__(self):
+        return "BlowupIdentity()"
+
+
+class BlowupCHV:
+    """kinetic.jl:70-95, the blow-up of arXiv:2210.00442: with x = |p| / sqrt(2 Ecut) the factor is 1 below x = 0.85,
+    Ecut/Ekin · Ca/(1-x)² from x = 0.9 on, and a C^∞ interpolation of x² and Ca/(1-x)² in between, so that the bands
+    become C² functions of k at a fixed cutoff (energy-cutoff smearing).  `p` is a NumPy array or a torch tensor."""
+    x1, x2 = 0.85, 0.90
+    Ca = 0.013952310177257383          # optimised to best match the x -> x² curve
+
+    def __call__(self, p, Ecut):
+        xp = _xp(p)
+        x = p / math.sqrt(2 * Ecut)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            ratio = Ecut / (p ** 2 / 2)
+            blow = self.Ca / (1 - x) ** 2
+            t = (x - self.x1) / (self.x2 - self.x1)
+            fa = xp.where(t > 0, xp.exp(-1 / xp.where(t > 0, t, 1.0)), 0.0)
+            fb = xp.where(1 - t > 0, xp.exp(-1 / xp.where(1 - t > 0, 1 - t, 1.0)), 0.0)
+            step = fa / (fa + fb)
+            mid = ratio * ((1 - step) * x ** 2 + step * blow)
+            return xp.where(x < self.x1, 1.0, xp.where(x < self.x2, mid, ratio * blow))
+
+    def __repr__(self):
+        return "BlowupCHV()"
+
+
+class BlowupAbinit:
+    """kinetic.jl:98-110, ABINIT's ecutsm: with Ecutsm = Ecutsm · Ecut the factor is 1 up to |p| = sqrt(2 (Ecut - Ecutsm))
+    and 1 / (x² (3 + x - 6x² + 3x²)) of x = (Ecut - |p|²/2) / Ecutsm above (the reference's polynomial as written)."""
+
+    def __init__(self, Ecutsm=0.5):
+        self.Ecutsm = float(Ecutsm)
+
+    def __call__(self, p, Ecut):
+        xp = _xp(p)
+        Ecutsm = Ecut * self.Ecutsm
+        assert Ecutsm < Ecut
+        x = (Ecut - p ** 2 / 2) / Ecutsm
+        with np.errstate(divide="ignore"):
+            return xp.where(p <= math.sqrt(2 * (Ecut - Ecutsm)), 1.0, 1 / (x ** 2 * (3 + x - 6 * x ** 2 + 3 * x ** 2)))
+
+    def __repr__(self):
+        return f"BlowupAbinit(Ecutsm={self.Ecutsm})"
+
+
+class Kinetic:
+    """kinetic.jl:7-12: the kinetic term with a scaling factor and a blow-up; a plain "Kinetic" is Kinetic()."""
+    name = "Kinetic"
+
+    def __init__(self, scaling_factor=1, blowup=None):
+        self.scaling_factor = scaling_factor
+        self.blowup = BlowupIdentity() if blowup is None else blowup
+
+    def __call__(self, basis):
+        return TermKinetic(basis, self.scaling_factor, self.blowup)
+
+    def __repr__(self):
+        return f"Kinetic(scaling_factor={self.scaling_factor}, blowup={self.blowup!r})"
+
+
+class TermKinetic:
+    """kinetic.jl:14-57: kinetic_energies[ik] = scaling_factor · |G+k|²/2 · blowup(|G+k|, Ecut), the table every device
+    path (Hψ, the preconditioners, band energies) reads from the k-block."""
+
+    def __init__(self, basis, scaling_factor=1.0, blowup=None):
         self.kinetic_energies = []
         for kpt in basis.kpoints:
             p = basis.Gplusk_vectors_cart(kpt)
-            self.kinetic_energies.append((scaling_factor * (p * p).sum(dim=1) / 2).contiguous())
+            ekin = (scaling_factor * (p * p).sum(dim=1) / 2)
+            if blowup is not None and not isinstance(blowup, BlowupIdentity):
+                ekin = ekin * blowup(p.norm(dim=1), basis.Ecut)
+            self.kinetic_energies.append(ekin.contiguous())
 
     def local_energy(self, basis, psi, occupation, **kw):
         """Σ over this rank's blocks (the mpi_sum of kinetic.jl:54 is done by the caller, packed with the other sums)."""
@@ -358,7 +434,31 @@ class TermXc:
         return E, [RealSpaceMultiplication(basis, k, pot[k.spin]) for k in basis.kpoints]
 
 
+def methfessel_paxton_order(kind):
+    """The order n of a ("MethfesselPaxton", n) smearing, None for every other kind."""
+    if isinstance(kind, (tuple, list)) and len(kind) == 2 and kind[0] == "MethfesselPaxton":
+        return kind[1]
+    return None
+
+
+def _mp_sums(n, x):
+    """Smearing.jl:133-168 for all of x at once: the A(i) H_k(x) sums of the Methfessel-Paxton occupation, entropy and
+    derivative, from the physicists' Hermite recursion H_k = 2x H_{k-1} - 2(k-1) H_{k-2} evaluated up to H_{2n}."""
+    H = [np.ones_like(x), 2 * x]
+    for k in range(2, 2 * n + 1):
+        H.append(2 * x * H[k - 1] - 2 * (k - 1) * H[k - 2])
+    A = [(-1) ** i / (math.factorial(i) * 4 ** i * math.sqrt(math.pi)) for i in range(n + 1)]
+    occ = sum((A[i] * H[2 * i - 1] for i in range(1, n + 1)), np.zeros_like(x))
+    ent = sum(A[i] * (H[2 * i] / 2 + (2 * i * H[2 * i - 2] if i else 0)) for i in range(n + 1))
+    der = sum(A[i] * H[2 * i] for i in range(n + 1))
+    return occ, ent, der
+
+
+_MV_SHIFT = 1 / math.sqrt(2)
+
+
 def smearing_occupation(kind, x):
+    """Smearing.occupation (Smearing.jl): f(x) with x = (ε - εF) / T; 1 at -∞ and 0 at +∞ for every kind."""
     x = np.asarray(x, dtype=float)
     if kind == "None":
         return np.where(x > 0, 0.0, 1.0)
@@ -367,10 +467,19 @@ def smearing_occupation(kind, x):
         return np.where(x > 0, ex / (1 + ex), 1 / (1 + ex))
     if kind == "Gaussian":
         return erfc(x) / 2
+    if kind == "MarzariVanderbilt":
+        u = x + _MV_SHIFT
+        return -erf(u) / 2 + np.exp(-u ** 2) / math.sqrt(2 * math.pi) + 0.5
+    n = methfessel_paxton_order(kind)
+    if n is not None:
+        xf = np.where(np.isinf(x), 0.0, x)
+        f = erfc(xf) / 2 + _mp_sums(n, xf)[0] * np.exp(-xf ** 2)
+        return np.where(np.isinf(x), np.where(x > 0, 0.0, 1.0), f)
     raise NotImplementedError(kind)
 
 
 def smearing_entropy(kind, x):
+    """Smearing.entropy: s(x) with s'(x) = x f'(x)."""
     x = np.asarray(x, dtype=float)
     if kind == "None":
         return np.zeros_like(x)
@@ -383,6 +492,31 @@ def smearing_entropy(kind, x):
         return out
     if kind == "Gaussian":
         return np.exp(-x ** 2) / (2 * math.sqrt(math.pi))
+    if kind == "MarzariVanderbilt":
+        u = x + _MV_SHIFT
+        return u * np.exp(-u ** 2) / math.sqrt(2 * math.pi)
+    n = methfessel_paxton_order(kind)
+    if n is not None:
+        return _mp_sums(n, x)[1] * np.exp(-x ** 2)
+    raise NotImplementedError(kind)
+
+
+def occupation_derivative(kind, x):
+    """Smearing.occupation_derivative in closed form: f'(x), an approximation of minus the delta function."""
+    x = np.asarray(x, dtype=float)
+    if kind == "None":
+        return np.zeros_like(x)
+    if kind == "FermiDirac":
+        ex = np.exp(-np.abs(x))
+        return -ex / (1 + ex) ** 2
+    if kind == "Gaussian":
+        return -np.exp(-x ** 2) / math.sqrt(math.pi)
+    if kind == "MarzariVanderbilt":
+        u = x + _MV_SHIFT
+        return -np.exp(-u ** 2) * (2 + math.sqrt(2) * x) / math.sqrt(math.pi)
+    n = methfessel_paxton_order(kind)
+    if n is not None:            # f' = -Σ_i A(i) H_2i(x) e^{-x²}, the order-n Hermite expansion of -δ
+        return -_mp_sums(n, x)[2] * np.exp(-x ** 2)
     raise NotImplementedError(kind)
 
 
