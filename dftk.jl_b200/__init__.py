@@ -77,3 +77,5 @@ from .scf import (self_consistent_field, next_density, AdaptiveBands, FixedBands
                   ScfConvergenceDensity, ScfConvergenceEnergy, SimpleMixing, KerkerMixing, LdosMixing, compute_ldos,
                   AndersonAcceleration, ScfDefaultCallback)
 from .direct_minimization import direct_minimization, select_occupied_orbitals
+from .transfer import (transfer_mapping, transfer_blochwave_kpt, transfer_blochwave, transfer_density, interpolate_density,
+                       apply_symop, unfold_bz, create_supercell, cell_to_supercell)

@@ -75,6 +75,11 @@ SIGNATURES = {
     "dftk_b200_tpa_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_vp]),
     "dftk_b200_real_dots_multi": (c_int, [c_i64, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "dftk_b200_axpy_dot_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_dbl, c_vp, c_i64, c_vp]),
+    "dftk_b200_remap_tables": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp]),
+    "dftk_b200_sphere_remap": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "dftk_b200_fourier_block_copy": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_i64]),
+    "dftk_b200_bspline2_prefilter": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_i64]),
+    "dftk_b200_bspline2_evaluate": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_i64, c_int]),
 }
 
 _lib = None

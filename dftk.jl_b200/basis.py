@@ -127,11 +127,13 @@ class Kpoint:
 class PlaneWaveBasis:
     def __init__(self, model, *, Ecut, kgrid=(1, 1, 1), kshift=(0, 0, 0), fft_size=None, supersampling=2.0,
                  architecture=None, comm_kpts=None, comm_slab=None, use_symmetries_for_kpoint_reduction=True,
-                 variational=True):
+                 variational=True, _symmetries_respect_rgrid=None):
         """`comm_kpts`: shard the (k, spin) blocks over the ranks (the reference's only distribution).
         `comm_slab`: instead, let ALL ranks work on every k-block together (single-k multi-GPU, e.g. a Γ-only supercell):
         the eigensolver cuts the plane-wave rows into one slab per rank (dftk_b200_lobpcg_slab), compute_density splits
-        the bands; everything else runs replicated on identical data."""
+        the bands; everything else runs replicated on identical data.
+        `_symmetries_respect_rgrid` (private): keep another basis's decision whether the symmetries must map the real-space
+        grid onto itself, although `fft_size` is passed (unfold_bz); None: True exactly when `fft_size` is None."""
         from .architecture import B200
         if not variational:
             raise NotImplementedError("Non-variational calculations are not supported")
@@ -147,7 +149,8 @@ class PlaneWaveBasis:
             raise ValueError("comm_slab needs an architecture whose context spans the same ranks (B200(comm=comm_slab))")
         dev = self.architecture.device
         self.kgrid = kgrid if isinstance(kgrid, (MonkhorstPack, ExplicitKpoints)) else MonkhorstPack(kgrid, kshift)
-        symmetries_respect_rgrid = fft_size is None
+        symmetries_respect_rgrid = fft_size is None if _symmetries_respect_rgrid is None else bool(_symmetries_respect_rgrid)
+        self.symmetries_respect_rgrid = symmetries_respect_rgrid
         if fft_size is None:
             dens = {Fraction(float(wi)).limit_denominator(12).denominator for s in model.symmetries for wi in s.w}
             factors = tuple(sorted({2, 3, 4, 6} & dens)) or (1,)
@@ -198,10 +201,7 @@ class PlaneWaveBasis:
         Gf = self.G_vectors.to(torch.float64)
         self.G_vectors_cart = Gf @ self._recip.T
 
-        def sphere(kcoord):          # Kpoint.jl:20-41: sphere membership over the whole cube
-            p = (Gf + torch.as_tensor(kcoord, device=dev)) @ self._recip.T
-            return (p * p).sum(dim=1) / 2 <= self.Ecut
-
+        sphere = self.sphere_mask
         costs = [1.0] * (n_kpt * n_spin)
         if comm.nranks > 1:          # every rank counts every sphere: the block -> rank map is identical everywhere
             npw = [float(sphere(k).sum().item()) for k in self.kcoords_global]
@@ -227,6 +227,11 @@ class PlaneWaveBasis:
         self.kblocks = _terms.build_kblocks(self)
 
     # ------------------------------------------------------------------ helpers
+    def sphere_mask(self, kcoord):
+        """Kpoint.jl:20-41: membership of every cube G in the kinetic-energy sphere of k-point `kcoord`."""
+        p = (self.G_vectors.to(torch.float64) + torch.as_tensor(kcoord, device=self.G_vectors.device)) @ self._recip.T
+        return (p * p).sum(dim=1) / 2 <= self.Ecut
+
     def Gplusk_vectors(self, kpt):
         return kpt.G_vectors.to(torch.float64) + torch.as_tensor(kpt.coordinate, device=kpt.G_vectors.device)
 

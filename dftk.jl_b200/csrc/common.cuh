@@ -145,6 +145,7 @@ struct dftk_b200_ctx {
   dftk::DevBuf<char> dm_items;
   dftk::DevBuf<double> dm_ws, dm_out, dm_w, dm_stats;
   dftk::DevBuf<dftk::cplx> dm_C, dm_M, dm_V;
+  dftk::DevBuf<char> tr_items;   // basis transfers (transfer.cu): descriptors of the pairs of one sphere remap
 };
 
 namespace dftk {

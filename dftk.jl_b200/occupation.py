@@ -171,14 +171,22 @@ def find_zero_secant_bisection(f, x, atol=np.finfo(float).eps, maxiters=1000):
     return x1
 
 
-def compute_occupation(basis, eigenvalues, *, fermialg=None, tol_n_elec=1e-6, gathered=None, return_global=False):
+def compute_occupation(basis, eigenvalues, *, fermialg=None, tol_n_elec=1e-6, gathered=None, return_global=False,
+                       eF=None):
     """Returns (occupation of the local blocks, εF).  `fermialg`: FermiBisection() or FermiTwoStage() (default:
     default_fermialg(model.smearing)).  `gathered` = (eigenvalues of all blocks, weights) when the caller already did
-    the allgather (next_density packs solver statistics into the same collective)."""
+    the allgather (next_density packs solver statistics into the same collective).  `eF` given: the occupations at that
+    Fermi level, without a search (occupation.jl, compute_occupation(basis, eigenvalues, εF))."""
     model = basis.model
     for ek in eigenvalues:
         if not np.all(np.diff(ek) >= -np.finfo(float).eps):
             raise ValueError("Eigenvalues should be monotonically increasing.")
+    if eF is not None:
+        occ = _occ(model, [np.asarray(e) for e in eigenvalues], eF)
+        if not return_global:
+            return occ, eF
+        ev = gathered[0] if gathered is not None else gather_eigenvalues(basis, eigenvalues)[0]
+        return occ, eF, _occ(model, ev, eF)
     ev, w = gathered if gathered is not None else gather_eigenvalues(basis, eigenvalues)[:2]
     filled = model.filled_occupation
     if model.n_electrons == 0:

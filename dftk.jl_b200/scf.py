@@ -399,8 +399,8 @@ def self_consistent_field(basis, *, rho=None, psi=None, tol=1e-6, is_converged=N
                 eigenvalues_global=info["eigenvalues_global"], occupation_global=info["occupation_global"],
                 n_iter=info["n_iter"], n_matvec=info["n_matvec"], history_Etot=info["history_Etot"],
                 history_drho=info["history_drho"], diagonalization=info["diagonalization"],
-                n_bands_converge=info["n_bands_converge"], runtime_s=time.time() - start, stage="finalize",
-                algorithm="SCF")
+                n_bands_converge=info["n_bands_converge"], occupation_threshold=nbandsalg.occupation_threshold,
+                runtime_s=time.time() - start, stage="finalize", algorithm="SCF")
 
 
 def ScfDefaultCallback():

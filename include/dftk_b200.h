@@ -297,6 +297,42 @@ int dftk_b200_real_dots_multi(int64_t n_pairs, int64_t n_blocks, dftk_b200_kbloc
 int dftk_b200_axpy_dot_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, void* const* Y, const void* const* X, double c,
                              const void* const* Z, int64_t n_bands, double* out_host);
 
+/* ---- moving data between plane-wave bases (src/transfer.jl, apply_symop of src/symmetry.jl:229-270, src/supercell.jl,
+ * src/interpolation.jl).  Orbital blocks are (n_bands, n_G) row-major complex128 device arrays (a band is a row); cubes are
+ * linear with x fastest.  None of these calls reads the k-block or grid objects: they take plain device arrays. */
+/* Tables of a sphere remap into a destination sphere of n_G integer vectors G (n_G x 3 int64, row-major, device):
+ *   H_j = G_j + delta,  idx[j] = lookup[cube index of M H_j] (-1 when M H_j is outside the nx x ny x nz source cube),
+ *   phase[j] = exp(-2 pi i H_j . tau)  (sincospi: rational tau with small denominators give exact +-1, +-i).
+ * M: 3x3 row-major integers, delta: 3 integers, tau: 3 doubles (all host; tau may be NULL when phase is NULL).  lookup: the
+ * source cube's nx*ny*nz int64 map cube index -> source row index, -1 outside the source sphere (device).  idx: n_G int64,
+ * phase: n_G complex128 or NULL (device).  Users: transfer to an equivalent k-point (M = I, delta = the lattice vector between
+ * the two k-points, tau = 0), apply_symop (M = S^-1, delta = the k shift that brings S k back to [-1/2, 1/2), tau), and
+ * the unit cell -> supercell map (M = I on the supercell's integer coordinates of k+G). */
+int dftk_b200_remap_tables(dftk_b200_ctx* ctx, int64_t n_G, const int64_t* G, const int32_t* M, const int32_t* delta,
+                           const double* tau, const int64_t* lookup, int nx, int ny, int nz, int64_t* idx, void* phase);
+/* Batched sphere remap, one launch for all n_pairs (source, destination) pairs (host arrays of n_pairs entries):
+ *   dst[p][row_offset[p] + b, j] = phase[p][j] * src[p][b, idx[p][j]]   for b < n_bands[p], j < n_dst[p],
+ * idx -1 giving 0 and a NULL phase (list or entry) giving 1.  ld_src / ld_dst: row lengths of the source and destination
+ * blocks; row_offset NULL = 0 (several sources may fill disjoint row ranges of one destination).  Destinations must not
+ * alias sources. */
+int dftk_b200_sphere_remap(dftk_b200_ctx* ctx, int64_t n_pairs, const void* const* src, const int64_t* ld_src, void* const* dst,
+                           const int64_t* ld_dst, const int64_t* row_offset, const int64_t* n_bands,
+                           const int64_t* const* idx, const int64_t* n_dst, const void* const* phase);
+/* Fourier block copy between cubes of different sizes (transfer_density; the blocks of transfer_mapping(basis_in, basis_out),
+ * transfer.jl:10-31, including its placement of the unmatched component of even sizes); every other output entry is zero.
+ * in: batch x (nx_in ny_in nz_in), out: batch x (nx_out ny_out nz_out), complex128 device. */
+int dftk_b200_fourier_block_copy(dftk_b200_ctx* ctx, const void* in, int nx_in, int ny_in, int nz_in, void* out, int nx_out,
+                                 int ny_out, int nz_out, int64_t batch);
+/* Prefilter of the periodic quadratic B-spline (Interpolations.jl BSpline(Quadratic(Periodic(OnCell())))) on Fourier
+ * coefficients, in place: f[b, m] /= prod_a (3/4 + cos(2 pi m_a / n_a) / 4)  (>= 1/8).  f: batch x N complex128 (device). */
+int dftk_b200_bspline2_prefilter(dftk_b200_ctx* ctx, void* f, int nx, int ny, int nz, int64_t batch);
+/* Evaluation of the periodic quadratic B-spline with coefficients f (batch x nx ny nz real, device) at the output points
+ * (i/nx_out, j/ny_out, k/nz_out) of a cell spanning rep[a] input cells along axis a (rep: 3 host integers, 1 1 1 for the same
+ * lattice): 27 taps per point, the tiling folded into the index arithmetic.  direct != 0 (needs n_out = rep * n_in on every
+ * axis): f holds the samples themselves and out is their periodic tiling.  out: batch x (nx_out ny_out nz_out) real (device). */
+int dftk_b200_bspline2_evaluate(dftk_b200_ctx* ctx, const double* f, int nx, int ny, int nz, const int32_t* rep, double* out,
+                                int nx_out, int ny_out, int nz_out, int64_t batch, int direct);
+
 #ifdef __cplusplus
 }
 #endif
