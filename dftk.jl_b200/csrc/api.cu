@@ -8,7 +8,7 @@ using namespace dftk;
 static std::string g_last_error;
 static std::mutex g_err_mutex;
 
-static int record(dftk_b200_ctx* ctx, int code, const std::string& msg) {
+int dftk::record_error(dftk_b200_ctx* ctx, int code, const std::string& msg) {
   {
     std::lock_guard<std::mutex> lk(g_err_mutex);
     g_last_error = msg;
@@ -16,14 +16,6 @@ static int record(dftk_b200_ctx* ctx, int code, const std::string& msg) {
   if (ctx) ctx->last_error = msg;
   return code;
 }
-
-#define API_BEGIN try {
-#define API_END(ctx)                                                        \
-  }                                                                         \
-  catch (const dftk::Error& e) { return record((ctx), e.code, e.what()); }  \
-  catch (const std::exception& e) { return record((ctx), DFTK_B200_EINVAL, e.what()); } \
-  catch (...) { return record((ctx), DFTK_B200_EINVAL, "unknown C++ exception"); }      \
-  return DFTK_B200_OK;
 
 // Stage a (possibly host) input buffer onto the device.  Returns a device pointer.
 static const void* stage_in(dftk_b200_ctx* ctx, const void* p, size_t bytes, DevBuf<char>& buf) {
@@ -629,7 +621,7 @@ int dftk_b200_apply_terms(dftk_b200_kblock* kb, const void* psi, void* hpsi, int
 }
 
 int dftk_b200_apply_h(dftk_b200_kblock* kb, const void* psi, void* hpsi, int64_t n_bands) {
-  if (!kb) return record(nullptr, DFTK_B200_EINVAL, "apply_h: kblock is NULL");
+  if (!kb) return record_error(nullptr, DFTK_B200_EINVAL, "apply_h: kblock is NULL");
   int parts = (kb->has_V ? 1 : 0) | (kb->has_kin ? 2 : 0) | (kb->n_nl() > 0 ? 4 : 0);
   return dftk_b200_apply_terms(kb, psi, hpsi, n_bands, parts, 0);
 }

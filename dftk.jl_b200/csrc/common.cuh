@@ -156,6 +156,17 @@ namespace dftk {
     CUDA_CHECK(cudaGetLastError());                                     \
   } while (0)
 
+// The error boundary of every extern "C" entry point: an exception becomes its error code, and its message is kept for
+// dftk_b200_last_error, per context and process-wide (the latter also answers calls that had no context).
+int record_error(dftk_b200_ctx* ctx, int code, const std::string& msg);   // api.cu
+#define API_BEGIN try {
+#define API_END(ctx)                                                                                \
+  }                                                                                                 \
+  catch (const ::dftk::Error& e) { return ::dftk::record_error((ctx), e.code, e.what()); }           \
+  catch (const std::exception& e) { return ::dftk::record_error((ctx), DFTK_B200_EINVAL, e.what()); } \
+  catch (...) { return ::dftk::record_error((ctx), DFTK_B200_EINVAL, "unknown C++ exception"); }      \
+  return DFTK_B200_OK;
+
 inline bool is_device_ptr(const void* p) {
   cudaPointerAttributes a;
   cudaError_t e = cudaPointerGetAttributes(&a, p);

@@ -154,26 +154,14 @@ void check_dev(int64_t n, const void* const* p, const char* what) {
   for (int64_t i = 0; i < n; ++i) REQUIRE(p[i] && is_device_ptr(p[i]), std::string(what) + ": orbitals must be device memory");
 }
 
-int fail(dftk_b200_ctx* ctx, int code, const char* msg) {
-  if (ctx) ctx->last_error = msg;
-  return code;
-}
-
 }  // namespace
-
-#define DM_BEGIN try {
-#define DM_END(ctx)                                                                   \
-  }                                                                                   \
-  catch (const dftk::Error& e) { return fail((ctx), e.code, e.what()); }              \
-  catch (const std::exception& e) { return fail((ctx), DFTK_B200_EINVAL, e.what()); } \
-  return DFTK_B200_OK;
 
 extern "C" {
 
 int dftk_b200_apply_h_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* psi, void* const* out,
                             int64_t n_bands, const double* scale_host) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "apply_h_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
   check_dev(n_blocks, psi, "apply_h_multi");
@@ -189,13 +177,13 @@ int dftk_b200_apply_h_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, cons
     LAUNCH(ctx, k_dm_scale, dim3(grid_for(ctx, mt), (unsigned)n_blocks), DM_THREADS, 0, put(ctx, ctx->dm_items, v));
     CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
   }
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_stiefel_project_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* X, void* const* G,
                                     int64_t n_bands) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "stiefel_project_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
   check_dev(n_blocks, X, "stiefel_project_multi");
@@ -207,13 +195,13 @@ int dftk_b200_stiefel_project_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   LAUNCH(ctx, k_dm_herm, (unsigned)n, DM_THREADS, 0, (const cplx*)C, M, nb);          // (X^H G + G^H X) / 2
   times(ctx, n, kbs, (const cplx* const*)X, M, nb, (cplx* const*)G, -1.0, 1.0);       // G -= X M
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_stiefel_retract_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* Y, void* const* X_out,
                                     int64_t n_bands) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "stiefel_retract_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
   check_dev(n_blocks, Y, "stiefel_retract_multi");
@@ -254,13 +242,13 @@ int dftk_b200_stiefel_retract_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   }
   times(ctx, n, kbs, (const cplx* const*)Y, S, nb, (cplx* const*)X_out, 1.0, 0.0);
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_tpa_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* X, const void* const* Q, void* const* S,
                         int64_t n_bands, const double* inv_w_host, int use_tpa, double* mean_kin) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "tpa_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
   REQUIRE(!use_tpa || (mean_kin && is_device_ptr(mean_kin)), "tpa_multi: mean_kin must be device memory");
@@ -285,13 +273,13 @@ int dftk_b200_tpa_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const vo
     LAUNCH(ctx, k_dm_tpa, dim3(grid_for(ctx, mt), (unsigned)n), DM_THREADS, 0, put(ctx, ctx->dm_items, v));
   }
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_real_dots_multi(int64_t n_pairs, int64_t n_blocks, dftk_b200_kblock* const* kbs, const void* const* A,
                               const void* const* B, int64_t n_bands, double* out_host) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "real_dots_multi");
   REQUIRE(n_pairs >= 1 && out_host, "real_dots_multi: bad argument");
   if (n_blocks == 0) {
@@ -307,13 +295,13 @@ int dftk_b200_real_dots_multi(int64_t n_pairs, int64_t n_blocks, dftk_b200_kbloc
       v.push_back(DmDotItem{(const cplx*)A[k], (const cplx*)B[k], nullptr, nullptr, 0.0, (long long)kbs[i]->n_pw * n_bands});
     }
   dots(ctx, v, (int)n_pairs, (int)n_blocks, out_host);
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_axpy_dot_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, void* const* Y, const void* const* X, double c,
                              const void* const* Z, int64_t n_bands, double* out_host) {
   dftk_b200_ctx* ctx = ctx_of(n_blocks, kbs);
-  DM_BEGIN
+  API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "axpy_dot_multi");
   if (out_host) *out_host = 0.0;
   if (n_blocks == 0) return DFTK_B200_OK;
@@ -328,7 +316,7 @@ int dftk_b200_axpy_dot_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, voi
     v.push_back(DmDotItem{Z ? (const cplx*)Z[i] : nullptr, (const cplx*)Y[i], (cplx*)Y[i], (const cplx*)X[i], c,
                           (long long)kbs[i]->n_pw * n_bands});
   dots(ctx, v, Z ? 1 : 0, (int)n_blocks, out_host);
-  DM_END(ctx)
+  API_END(ctx)
 }
 
 }  // extern "C"

@@ -2,7 +2,7 @@
 // src/eigen/lobpcg_hyper_impl.jl:354-582 (LOBPCG with B = I), :141-171 (rayleigh_ritz), :216-261
 // (ortho!), :271-323 (ortho!(X,Y,BY)), :190-210 (safe_cholesky), :264-268 (drop_small!) and the TPA
 // preconditioner of src/eigen/preconditioners.jl:27-78, with Julia's active-block views expressed as
-// column offsets.  All N_pw-sized work is GEMMs (blas.cu) or fused elementwise kernels below; the small
+// column offsets.  All N_pw-sized work is GEMMs (blas.cu) or fused elementwise kernels (lobpcg_batch.cuh); the small
 // dense factorisations (<= 3M x 3M) use cuSOLVER (heevd / potrf / trtri), as SURVEY.md §7 allows.
 #include <algorithm>
 #include <cfloat>
@@ -25,107 +25,11 @@ struct Mat {
   Mat cols_range(int64_t c0, int64_t nc) const { return Mat{p + ld * c0, ld, rows, nc}; }
 };
 
-// ------------------------------------------------------------------ small kernels
-__global__ void k_residual(const cplx* __restrict__ AX, const cplx* __restrict__ X,
-                           const double* __restrict__ lam, cplx* __restrict__ R, int64_t ld,
-                           int64_t n_rows, const double* __restrict__ kin, double* __restrict__ norms,
-                           double* __restrict__ meankin, int squared) {
-  // one CTA per column: R = AX - X*lam; norms = ||R||; meankin = <X|kin|X>   (:443-445, precondprep!)
-  // squared != 0: norms = ||R||^2 of this rank's rows (slab solves: summed over the ranks, then k_sqrt_n)
-  const int64_t col = blockIdx.x;
-  const cplx* ax = AX + ld * col;
-  const cplx* x = X + ld * col;
-  cplx* r = R + ld * col;
-  const double l = lam[col];
-  double s = 0.0, mk = 0.0;
-  for (int64_t i = threadIdx.x; i < n_rows; i += blockDim.x) {
-    cplx a = ax[i], b = x[i];
-    cplx v = make_double2(a.x - l * b.x, a.y - l * b.y);
-    r[i] = v;
-    s += v.x * v.x + v.y * v.y;
-    if (kin) mk += kin[i] * (b.x * b.x + b.y * b.y);
-  }
-  __shared__ double rs[32], rm[32];
-  for (int o = 16; o > 0; o >>= 1) {
-    s += __shfl_down_sync(0xffffffffu, s, o);
-    mk += __shfl_down_sync(0xffffffffu, mk, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    rs[threadIdx.x >> 5] = s;
-    rm[threadIdx.x >> 5] = mk;
-  }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    int nw = blockDim.x >> 5;
-    s = threadIdx.x < nw ? rs[threadIdx.x] : 0.0;
-    mk = threadIdx.x < nw ? rm[threadIdx.x] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) {
-      s += __shfl_down_sync(0xffffffffu, s, o);
-      mk += __shfl_down_sync(0xffffffffu, mk, o);
-    }
-    if (threadIdx.x == 0) {
-      norms[col] = squared ? s : sqrt(s);
-      meankin[col] = mk;
-    }
-  }
-}
-
-// R[:,n] *= mk_n / (mk_n + kin)    (ldiv!(::PreconditionerTPA), src/gpu/linalg.jl:29-36)
-__global__ void k_precondition(cplx* __restrict__ R, int64_t ld, int64_t n_rows, int64_t n_cols,
-                               const double* __restrict__ kin, const double* __restrict__ meankin) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_rows * n_cols) return;
-  int64_t i = idx % n_rows, c = idx / n_rows;
-  double mk = meankin[c];
-  double f = mk / (mk + kin[i]);
-  cplx v = R[i + ld * c];
-  R[i + ld * c] = make_double2(v.x * f, v.y * f);
-}
-
+// ------------------------------------------------------------------ small kernels of the direct path only
 __global__ void k_sqrt_n(double* __restrict__ v, int64_t n) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) v[i] = sqrt(v[i]);
 }
-__global__ void k_col_norms(const cplx* __restrict__ X, int64_t ld, int64_t n_rows,
-                            double* __restrict__ norms, int squared) {
-  const int64_t col = blockIdx.x;
-  const cplx* x = X + ld * col;
-  double s = 0.0;
-  for (int64_t i = threadIdx.x; i < n_rows; i += blockDim.x) {
-    cplx v = x[i];
-    s += v.x * v.x + v.y * v.y;
-  }
-  __shared__ double rs[32];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) rs[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    int nw = blockDim.x >> 5;
-    s = threadIdx.x < nw ? rs[threadIdx.x] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-    if (threadIdx.x == 0) norms[col] = squared ? s : sqrt(s);
-  }
-}
-
-__global__ void k_scale_cols_inv(cplx* __restrict__ X, int64_t ld, int64_t n_rows, int64_t n_cols,
-                                 const double* __restrict__ norms) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_rows * n_cols) return;
-  int64_t i = idx % n_rows, c = idx / n_rows;
-  double f = 1.0 / norms[c];
-  cplx v = X[i + ld * c];
-  X[i + ld * c] = make_double2(v.x * f, v.y * f);
-}
-
-// strided 2D copy (dst and src column-major with different leading dimensions)
-__global__ void k_copy2d(cplx* __restrict__ dst, int64_t ldd, const cplx* __restrict__ src, int64_t lds,
-                         int64_t n_rows, int64_t n_cols) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_rows * n_cols) return;
-  int64_t i = idx % n_rows, c = idx / n_rows;
-  dst[i + ldd * c] = src[i + lds * c];
-}
-
 // Hermitian(upper): mirror the strictly upper triangle into the lower one, make the diagonal real
 __global__ void k_hermitize_upper(cplx* __restrict__ A, int64_t ld, int64_t n) {
   int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -147,77 +51,6 @@ __global__ void k_zero_lower(cplx* __restrict__ A, int64_t ld, int64_t n) {
 __global__ void k_add_diag(cplx* __restrict__ A, int64_t ld, int64_t n, double shift) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) A[i + ld * i].x += shift;
-}
-// cP = cX[:, c0:] - e,  e[newly_locked + c, c] = 1 for c < lenXn   (lobpcg_hyper_impl.jl:495-503)
-__global__ void k_make_cP(cplx* __restrict__ cP, const cplx* __restrict__ cX, int64_t ld, int64_t n_rows,
-                          int64_t n_cols, int64_t c0, int64_t lenXn) {
-  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_rows * n_cols) return;
-  int64_t i = idx % n_rows, c = idx / n_rows;
-  int64_t cc = c + c0;  // column in cX / e
-  cplx v = cX[i + ld * cc];
-  if (cc < lenXn && i == c0 + cc) v.x -= 1.0;
-  cP[i + ld * c] = v;
-}
-
-// stats[0] = max |diag|, stats[1] = sum |offdiag|^2, stats[2] = #nan/inf, stats[3] = sum |all|^2
-__global__ void k_matrix_stats(const cplx* __restrict__ A, int64_t ld, int64_t n_rows, int64_t n_cols,
-                               double* __restrict__ stats) {
-  // single CTA (matrices are small): deterministic
-  double md = 0.0, so = 0.0, bad = 0.0, sa = 0.0;
-  for (int64_t idx = threadIdx.x; idx < n_rows * n_cols; idx += blockDim.x) {
-    int64_t i = idx % n_rows, j = idx / n_rows;
-    cplx v = A[i + ld * j];
-    double a2 = v.x * v.x + v.y * v.y;
-    if (!isfinite(a2)) bad += 1.0;
-    sa += a2;
-    if (i == j) md = fmax(md, sqrt(a2));
-    else so += a2;
-  }
-  __shared__ double r0[32], r1[32], r2[32], r3[32];
-  for (int o = 16; o > 0; o >>= 1) {
-    md = fmax(md, __shfl_down_sync(0xffffffffu, md, o));
-    so += __shfl_down_sync(0xffffffffu, so, o);
-    bad += __shfl_down_sync(0xffffffffu, bad, o);
-    sa += __shfl_down_sync(0xffffffffu, sa, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    r0[threadIdx.x >> 5] = md;
-    r1[threadIdx.x >> 5] = so;
-    r2[threadIdx.x >> 5] = bad;
-    r3[threadIdx.x >> 5] = sa;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int nw = blockDim.x >> 5;
-    for (int w = 1; w < nw; ++w) {
-      md = fmax(md, r0[w]);
-      so += r1[w];
-      bad += r2[w];
-      sa += r3[w];
-    }
-    stats[0] = md;
-    stats[1] = so;
-    stats[2] = bad;
-    stats[3] = sa;
-  }
-}
-
-// counter-based normal random numbers (for drop_small!'s re-randomisation; statistically plain)
-__device__ __forceinline__ uint64_t splitmix(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-__global__ void k_randn_col(cplx* __restrict__ x, int64_t n_rows, uint64_t seed) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_rows) return;
-  uint64_t a = splitmix(seed + 2 * (uint64_t)i), b = splitmix(seed + 2 * (uint64_t)i + 1);
-  double u1 = ((a >> 11) + 1.0) * (1.0 / 9007199254740993.0);
-  double u2 = (b >> 11) * (1.0 / 9007199254740992.0);
-  double r = sqrt(-2.0 * log(u1));
-  x[i] = make_double2(r * cospi(2.0 * u2) * 0.70710678118654752, r * sinpi(2.0 * u2) * 0.70710678118654752);
 }
 __global__ void k_compute_lambda(const cplx* __restrict__ num, const cplx* __restrict__ den,
                                  double* __restrict__ lam, int64_t n) {
@@ -362,6 +195,42 @@ static void coro_entry() {
   swapcontext(&c->uc, g_main_uc);
 }
 static inline void coro_yield(Coro* c) { swapcontext(&c->uc, g_main_uc); }
+
+static void small_gram_geometry(dftk_b200_ctx* ctx, int64_t rows, int* n_ctas_out, long long* rpc_out) {
+  int64_t n_ctas = std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, 2 * (int64_t)ctx->sm_count));
+  int64_t rpc = (rows + n_ctas - 1) / n_ctas;
+  rpc = (rpc + SMALL_TR - 1) / SMALL_TR * SMALL_TR;
+  n_ctas = std::max<int64_t>(1, (rows + rpc - 1) / rpc);
+  *n_ctas_out = (int)n_ctas;
+  *rpc_out = rpc;
+}
+// One Gram item C = A' B of single tall blocks, with the CTA geometry of the batched kernel.
+static GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB,
+                                 int64_t n_rows, cplx* C) {
+  GramItem g{};
+  g.A.n = g.B.n = 1;
+  g.A.p[0] = A; g.A.ld[0] = lda; g.A.cols[0] = nA;
+  g.B.p[0] = B; g.B.ld[0] = ldb; g.B.cols[0] = nB;
+  for (int q = 1; q < 4; ++q) { g.A.start[q] = nA; g.B.start[q] = nB; }
+  g.n_rows = n_rows;
+  small_gram_geometry(ctx, n_rows, &g.n_ctas, &g.rows_per_cta);
+  g.upper_only = 0;
+  g.C = C;
+  g.ldc = nA;
+  return g;
+}
+// One update item out = alpha Y c + beta out of a single tall block Y (n_rows x nY, like out of leading dimension n_rows;
+// c is nY x ncols, packed).
+static BtimesItem single_btimes_item(const cplx* Y, int nY, const cplx* c, int ncols, cplx* out, int64_t n_rows, double alpha,
+                                     double beta) {
+  BtimesItem b{};
+  b.Y.n = 1;
+  b.Y.p[0] = Y; b.Y.ld[0] = n_rows; b.Y.cols[0] = nY;
+  for (int q = 1; q < 4; ++q) b.Y.start[q] = nY;
+  b.cm = c; b.ldcm = nY; b.ncols = ncols;
+  b.out = out; b.ldo = n_rows; b.n_rows = n_rows; b.alpha = alpha; b.beta = beta;
+  return b;
+}
 
 // Launches the recorded operations: the same operation of several solves becomes one launch.
 struct BatchExec {
@@ -610,24 +479,9 @@ struct BatchExec {
             continue;
           }
           cplx* proj = kb->proj.ensure((size_t)2 * kb->n_nl() * SMALL_MAX_N);
-          GramItem gi{};
-          gi.A.n = gi.B.n = 1;
-          gi.A.p[0] = kb->P.p; gi.A.ld[0] = kb->n_pw; gi.A.cols[0] = (int)kb->n_nl();
-          gi.B.p[0] = a.in; gi.B.ld[0] = kb->n_pw; gi.B.cols[0] = a.ncols;
-          for (int q = 1; q < 4; ++q) { gi.A.start[q] = (int)kb->n_nl(); gi.B.start[q] = a.ncols; }
-          gi.n_rows = kb->n_pw;
-          small_gram_geometry(ctx, kb->n_pw, &gi.n_ctas, &gi.rows_per_cta);
-          gi.upper_only = 0;
-          gi.C = proj;
-          gi.ldc = kb->n_nl();
-          g.push_back(gi);
-          BtimesItem bi{};
-          bi.Y.n = 1;
-          bi.Y.p[0] = kb->PD.p; bi.Y.ld[0] = kb->n_pw; bi.Y.cols[0] = (int)kb->n_nl();
-          for (int q = 1; q < 4; ++q) bi.Y.start[q] = (int)kb->n_nl();
-          bi.cm = proj; bi.ldcm = kb->n_nl(); bi.ncols = a.ncols;
-          bi.out = a.out; bi.ldo = kb->n_pw; bi.n_rows = kb->n_pw; bi.alpha = 1.0; bi.beta = 1.0;
-          b.push_back(bi);
+          const int nl = (int)kb->n_nl();
+          g.push_back(single_gram_item(ctx, kb->P.p, kb->n_pw, nl, a.in, kb->n_pw, a.ncols, kb->n_pw, proj));
+          b.push_back(single_btimes_item(kb->PD.p, nl, proj, a.ncols, a.out, kb->n_pw, 1.0, 1.0));
         }
         if (!g.empty()) {
           gram_batch(g);
@@ -650,15 +504,6 @@ struct BatchExec {
       default: throw Error(DFTK_B200_EINVAL, "batched LOBPCG: unknown operation");
     }
   }
-  static void small_gram_geometry(dftk_b200_ctx* ctx, int64_t rows, int* n_ctas_out, long long* rpc_out) {
-    int64_t n_ctas = std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, 2 * (int64_t)ctx->sm_count));
-    int64_t rpc = (rows + n_ctas - 1) / n_ctas;
-    rpc = (rpc + SMALL_TR - 1) / SMALL_TR * SMALL_TR;
-    n_ctas = std::max<int64_t>(1, (rows + rpc - 1) / rpc);
-    *n_ctas_out = (int)n_ctas;
-    *rpc_out = rpc;
-  }
-
   // run everything recorded by the solves since the last round; one stream synchronisation at the end
   void flush(std::vector<Coro*>& coros) {
     issue(coros);
@@ -859,7 +704,7 @@ struct Lobpcg {
     g.B = mklist(B);
     if (g.A.start[g.A.n] == 0 || g.B.start[g.B.n] == 0) return;
     g.n_rows = A[0].rows;
-    BatchExec::small_gram_geometry(ctx, g.n_rows, &g.n_ctas, &g.rows_per_cta);
+    small_gram_geometry(ctx, g.n_rows, &g.n_ctas, &g.rows_per_cta);
     g.upper_only = upper_only ? 1 : 0;
     g.C = C;
     g.ldc = ldc;
@@ -875,15 +720,21 @@ struct Lobpcg {
     newop(OP_BTIMES).u.btimes = b;
   }
 
-  void copy2d(Mat dst, Mat src) {
-    if (src.rows == 0 || src.cols == 0) return;
+  // One block operation of lobpcg_batch.cuh: recorded for the batched launch on the small path, launched on its own
+  // otherwise (k_item on grid x block threads, the item passed as the kernel parameter)
+  template <class Item>
+  void block_op(int type, Item Op::U::*slot, const Item& it, unsigned grid, unsigned block = 256) {
     if (small) {
-      newop(OP_COPY2D).u.copy2d = Copy2dItem{dst.p, dst.ld, src.p, src.ld, src.rows, (int)src.cols};
+      newop(type).u.*slot = it;
       return;
     }
+    LAUNCH(ctx, k_item<Item>, grid, block, 0, it);
+  }
+
+  void copy2d(Mat dst, Mat src) {
+    if (src.rows == 0 || src.cols == 0) return;
     touch(dst.p, dst.ld * src.cols);
-    LAUNCH(ctx, k_copy2d, nblk(src.rows * src.cols), 256, 0, dst.p, dst.ld, (const cplx*)src.p, src.ld,
-           src.rows, src.cols);
+    block_op(OP_COPY2D, &Op::U::copy2d, Copy2dItem{dst.p, dst.ld, src.p, src.ld, src.rows, (int)src.cols}, nblk(src.rows * src.cols));
   }
   // contiguous device copy / zero fill of `n` complex numbers
   void copy_flat(cplx* dst, const cplx* src, int64_t n) {
@@ -898,12 +749,8 @@ struct Lobpcg {
   }
   void col_norms(Mat X, double* out) {
     if (X.cols == 0) return;
-    if (small) {
-      newop(OP_COLNORMS).u.colnorm = ColnormItem{X.p, X.ld, X.rows, (int)X.cols, out};
-      return;
-    }
-    const bool dist = is_dist(X.rows);
-    LAUNCH(ctx, k_col_norms, (unsigned)X.cols, 256, 0, (const cplx*)X.p, X.ld, X.rows, out, dist ? 1 : 0);
+    const bool dist = is_dist(X.rows);     // slab rows: squared norms, summed over the ranks
+    block_op(OP_COLNORMS, &Op::U::colnorm, ColnormItem{X.p, X.ld, X.rows, (int)X.cols, dist, out}, (unsigned)X.cols);
     if (dist) {
       reduce(out, (size_t)X.cols);
       LAUNCH(ctx, k_sqrt_n, nblk(X.cols), 256, 0, out, X.cols);
@@ -911,27 +758,16 @@ struct Lobpcg {
   }
   void scale_cols_inv(Mat X, const double* norms) {
     if (X.cols == 0) return;
-    if (small) {
-      newop(OP_SCALE).u.scale = ScaleItem{X.p, X.ld, X.rows, (int)X.cols, norms};
-      return;
-    }
     touch(X);
-    LAUNCH(ctx, k_scale_cols_inv, nblk(X.rows * X.cols), 256, 0, X.p, X.ld, X.rows, X.cols, norms);
+    block_op(OP_SCALE, &Op::U::scale, ScaleItem{X.p, X.ld, X.rows, (int)X.cols, norms}, nblk(X.rows * X.cols));
   }
   void matrix_stats(const cplx* A, int64_t ld, int64_t r, int64_t c, double* out) {
-    if (small) {
-      newop(OP_STATS).u.stats = StatsItem{A, ld, (int)r, (int)c, out};
-      return;
-    }
-    LAUNCH(ctx, k_matrix_stats, 1, 1024, 0, A, ld, r, c, out);
+    block_op(OP_STATS, &Op::U::stats, StatsItem{A, ld, (int)r, (int)c, out}, 1, 1024);
   }
   void randn_col(cplx* x, int64_t n_rows, uint64_t seed) {
-    if (small) {
-      newop(OP_RANDN).u.randn = RandnItem{x, n_rows, seed};
-      return;
-    }
     touch(x, n_rows);
-    LAUNCH(ctx, k_randn_col, nblk(n_rows), 256, 0, x, n_rows, seed + (is_dist(n_rows) ? 2 * (uint64_t)row0 : 0));   // slabs: one global random column
+    const uint64_t s = seed + (is_dist(n_rows) ? 2 * (uint64_t)row0 : 0);   // slabs: one global random column
+    block_op(OP_RANDN, &Op::U::randn, RandnItem{x, n_rows, s}, nblk(n_rows));
   }
   void stats(const cplx* A, int64_t ld, int64_t r, int64_t c, double* out4) {
     matrix_stats(A, ld, r, c, d_stats);
@@ -1332,13 +1168,13 @@ void Lobpcg::apply_h_slab(Mat in, Mat out) {
   if (my_nc > 0) {
     for (int r = 0; r < R; ++r) {
       const int64_t nr = row_off[r + 1] - row_off[r];
-      LAUNCH(ctx, k_copy2d, nblk(nr * my_nc), 256, 0, slab_in + row_off[r], Nfull, (const cplx*)(slab_stage + row_off[r] * my_nc), nr, nr, my_nc);
+      copy2d(Mat{slab_in + row_off[r], Nfull, nr, my_nc}, Mat{slab_stage + row_off[r] * my_nc, nr, nr, my_nc});
     }
     kb_apply_local_kinetic(kb, slab_in, slab_out, my_nc, kb->has_V, kb->has_kin, false);
     kb_apply_nonlocal(kb, slab_in, slab_out, my_nc);
     for (int r = 0; r < R; ++r) {
       const int64_t nr = row_off[r + 1] - row_off[r];
-      LAUNCH(ctx, k_copy2d, nblk(nr * my_nc), 256, 0, slab_stage + row_off[r] * my_nc, nr, (const cplx*)(slab_out + row_off[r]), Nfull, nr, my_nc);
+      copy2d(Mat{slab_stage + row_off[r] * my_nc, nr, nr, my_nc}, Mat{slab_out + row_off[r], Nfull, nr, my_nc});
     }
   }
   slab_t_apply += tick();
@@ -1475,36 +1311,25 @@ void Lobpcg::body(SolveArgs& a) {
     }
     prof.begin("residual+precond");
     // residuals :443-445 (+ precondprep! :452-457 fused)
-    if (small) {
-      newop(OP_RESIDUAL).u.residual = ResidualItem{nAX + N * a0, nX + N * a0, d_lam + a0, nR + N * a0, N, N, (int)Ma,
-                                                   use_prec ? kb->kin.p : nullptr, d_norms, d_meankin};
-      // one read-back: the residual norms and the status of the Jacobi eigensolver of this Rayleigh-Ritz step
-      const size_t span = (size_t)(d_stats - d_norms) + 8;
-      std::vector<double> both(span);
-      get(both.data(), d_norms, span * sizeof(double));
-      std::copy(both.begin(), both.begin() + Ma, norms.begin());
-      if (niter > 0 && both[(d_stats - d_norms) + 4] == 0.0)
-        throw Error(DFTK_B200_ENUM, "rayleigh_ritz: Jacobi eigensolver did not converge");
-    } else {
-      touch(nR + N * a0, N * Ma);
-      LAUNCH(ctx, k_residual, (unsigned)Ma, 256, 0, (const cplx*)(nAX + N * a0), (const cplx*)(nX + N * a0),
-             (const double*)(d_lam + a0), nR + N * a0, N, N, use_prec ? kinp() : nullptr,
-             d_norms, d_meankin, slab ? 1 : 0);
-      if (slab) {
-        reduce(d_norms, (size_t)(M + Ma));          // [d_norms, d_norms + M) and the Ma entries of d_meankin behind it
-        LAUNCH(ctx, k_sqrt_n, nblk(Ma), 256, 0, d_norms, Ma);
-      }
-      get(norms.data(), d_norms, Ma * sizeof(double));
+    touch(nR + N * a0, N * Ma);
+    block_op(OP_RESIDUAL, &Op::U::residual, ResidualItem{nAX + N * a0, nX + N * a0, d_lam + a0, nR + N * a0, N, N, (int)Ma, slab,
+                                                         use_prec ? kinp() : nullptr, d_norms, d_meankin}, (unsigned)Ma);
+    if (slab) {
+      reduce(d_norms, (size_t)(M + Ma));          // [d_norms, d_norms + M) and the Ma entries of d_meankin behind it
+      LAUNCH(ctx, k_sqrt_n, nblk(Ma), 256, 0, d_norms, Ma);
+    }
+    {
+      // one read-back: the residual norms and, on the small path, the status of the Jacobi eigensolver of this Rayleigh-Ritz step
+      const size_t jacobi = (size_t)(d_stats - d_norms) + 4;
+      std::vector<double> back(small ? jacobi + 4 : (size_t)Ma);
+      get(back.data(), d_norms, back.size() * sizeof(double));
+      std::copy(back.begin(), back.begin() + Ma, norms.begin());
+      if (small && niter > 0 && back[jacobi] == 0.0) throw Error(DFTK_B200_ENUM, "rayleigh_ritz: Jacobi eigensolver did not converge");
     }
     for (int64_t i = 0; i < Ma; ++i) RH(a0 + i, niter) = norms[i];
     if (use_prec) {
-      if (small) {
-        newop(OP_PRECOND).u.precond = PrecondItem{nR + N * a0, N, N, (int)Ma, kb->kin.p, d_meankin};
-      } else {
-        touch(nR + N * a0, N * Ma);
-        LAUNCH(ctx, k_precondition, nblk(N * Ma), 256, 0, nR + N * a0, N, N, Ma, kinp(),
-               (const double*)d_meankin);
-      }
+      touch(nR + N * a0, N * Ma);
+      block_op(OP_PRECOND, &Op::U::precond, PrecondItem{nR + N * a0, N, N, (int)Ma, kinp(), d_meankin}, nblk(N * Ma));
     }
 
     const int64_t prev_nlocked = nlocked;
@@ -1526,11 +1351,8 @@ void Lobpcg::body(SolveArgs& a) {
       const int64_t lenXn = Ma - newly;
       prof.begin("cP ortho");
       // cP = (cX - e)[:, newly:Ma]; ortho!(cP, cX, cX)
-      if (small) {
-        newop(OP_MAKECP).u.makecp = MakecpItem{cP, cX, S3, (int)ncolsY, (int)lenXn, (int)newly, (int)lenXn};
-      } else {
-        LAUNCH(ctx, k_make_cP, nblk(ncolsY * lenXn), 256, 0, cP, (const cplx*)cX, S3, ncolsY, lenXn, newly, lenXn);
-      }
+      block_op(OP_MAKECP, &Op::U::makecp, MakecpItem{cP, cX, S3, (int)ncolsY, (int)lenXn, (int)newly, (int)lenXn},
+               nblk(ncolsY * lenXn));
       ortho_against(Mat{cP, S3, ncolsY, lenXn}, {Mat{cX, S3, ncolsY, Ma}}, G, S3);
       prof.begin("P,AP = Y cP");
       blocks_times(Y, cP, S3, lenXn, mat(nP).cols_from(a0 + newly), 1.0, 0.0);
@@ -1761,8 +1583,10 @@ void random_orbitals_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, cplx*
     A[i] = SolveArgs{Xs[i], 0, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr};
     L[i].prepare(A[i]);
     const uint64_t s = seed * 0x9E3779B97F4A7C15ull + ((uint64_t)i << 40);
-    for (int64_t c = 0; c < M; ++c)
-      LAUNCH(ctx, k_randn_col, nblk(L[i].N), 256, 0, Xs[i] + L[i].N * c, L[i].N, s + ((uint64_t)c << 24) * 2654435761ull);
+    for (int64_t c = 0; c < M; ++c) {
+      const RandnItem col{Xs[i] + L[i].N * c, L[i].N, s + ((uint64_t)c << 24) * 2654435761ull};
+      LAUNCH(ctx, k_item<RandnItem>, nblk(L[i].N), 256, 0, col);
+    }
   }
   if (!L[0].small) {
     for (int64_t i = 0; i < n_blocks; ++i) L[i].ortho(Mat{Xs[i], L[i].N, L[i].N, M}, L[i].tmpN, L[i].N);
@@ -1813,16 +1637,7 @@ void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* co
         for (int b = 0; b < nb; ++b) enl_host[i * ld_out + b] = 0.0;
       } else {
         cplx* proj = kb->proj.ensure((size_t)2 * kb->n_proj * SMALL_MAX_N);
-        GramItem g{};
-        g.A.n = g.B.n = 1;
-        g.A.p[0] = kb->P.p; g.A.ld[0] = kb->n_pw; g.A.cols[0] = (int)kb->n_proj;
-        g.B.p[0] = psi[i]; g.B.ld[0] = kb->n_pw; g.B.cols[0] = nb;
-        for (int q = 1; q < 4; ++q) { g.A.start[q] = (int)kb->n_proj; g.B.start[q] = nb; }
-        g.n_rows = kb->n_pw;
-        BatchExec::small_gram_geometry(ctx, kb->n_pw, &g.n_ctas, &g.rows_per_cta);
-        g.C = proj;
-        g.ldc = kb->n_proj;
-        gr.push_back(g);
+        gr.push_back(single_gram_item(ctx, kb->P.p, kb->n_pw, (int)kb->n_proj, psi[i], kb->n_pw, nb, kb->n_pw, proj));
         ne.push_back(NlEnergyItem{proj, kb->Dc.p, (int)kb->n_proj, nb, sc + SMALL_MAX_N});
         ga.push_back(GatherItem{sc + SMALL_MAX_N, nb, (int)used});
         scatter.push_back({enl_host + i * ld_out, {used, nb}});
@@ -1896,16 +1711,7 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
     n_spin = std::max(n_spin, kb->spin + 1);
     cplx* a = kb->proj.ensure((size_t)n_orb * std::max(nb, SMALL_MAX_N));
     if (nb <= SMALL_MAX_N && n_orb <= SMALL_MAX_COLS) {
-      GramItem g{};
-      g.A.n = g.B.n = 1;
-      g.A.p[0] = kb->P.p + kb->n_pw * kb->n_proj; g.A.ld[0] = kb->n_pw; g.A.cols[0] = (int)n_orb;
-      g.B.p[0] = psi[i]; g.B.ld[0] = kb->n_pw; g.B.cols[0] = nb;
-      for (int q = 1; q < 4; ++q) { g.A.start[q] = (int)n_orb; g.B.start[q] = nb; }
-      g.n_rows = kb->n_pw;
-      BatchExec::small_gram_geometry(ctx, kb->n_pw, &g.n_ctas, &g.rows_per_cta);
-      g.C = a;
-      g.ldc = n_orb;
-      gr.push_back(g);
+      gr.push_back(single_gram_item(ctx, kb->P.p + kb->n_pw * kb->n_proj, kb->n_pw, (int)n_orb, psi[i], kb->n_pw, nb, kb->n_pw, a));
     } else {
       kb_project_cols(kb, kb->n_proj, n_orb, psi[i], nb, a);
     }
@@ -1923,22 +1729,6 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
 // C (nA x nB, host, column-major) = A' B for tall column-major blocks (n_rows >> nA, nB <= SMALL_MAX_COLS): one fused launch
 // (CTA partials + last-CTA reduction, lobpcg_small.cuh).  Used by the host driver for the history dot products of Anderson
 // mixing (src/scf/anderson.jl:81-130) instead of a QR factorisation of the N_fft x m history matrix.
-// One Gram item C = A' B of single tall blocks, with the CTA geometry of the batched kernel.
-static GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB,
-                                 int64_t n_rows, cplx* C) {
-  GramItem g{};
-  g.A.n = g.B.n = 1;
-  g.A.p[0] = A; g.A.ld[0] = lda; g.A.cols[0] = nA;
-  g.B.p[0] = B; g.B.ld[0] = ldb; g.B.cols[0] = nB;
-  for (int q = 1; q < 4; ++q) { g.A.start[q] = nA; g.B.start[q] = nB; }
-  g.n_rows = n_rows;
-  BatchExec::small_gram_geometry(ctx, n_rows, &g.n_ctas, &g.rows_per_cta);
-  g.upper_only = 0;
-  g.C = C;
-  g.ldc = nA;
-  return g;
-}
-
 void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
                cplx* out_host) {
   REQUIRE(nA >= 1 && nB >= 1 && nA <= SMALL_MAX_COLS && nB <= SMALL_MAX_COLS, "tall_gram: 1 <= columns <= 96");
@@ -1970,15 +1760,7 @@ void dm_small_times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, con
   REQUIRE(nb <= SMALL_MAX_N, "dm_small_times: too many bands");
   BatchExec exec(ctx);
   std::vector<BtimesItem> v;
-  for (int i = 0; i < n; ++i) {
-    BtimesItem b{};
-    b.Y.n = 1;
-    b.Y.p[0] = Y[i]; b.Y.ld[0] = kbs[i]->n_pw; b.Y.cols[0] = nb;
-    for (int q = 1; q < 4; ++q) b.Y.start[q] = nb;
-    b.cm = M + (size_t)i * nb * nb; b.ldcm = nb; b.ncols = nb;
-    b.out = out[i]; b.ldo = kbs[i]->n_pw; b.n_rows = kbs[i]->n_pw; b.alpha = alpha; b.beta = beta;
-    v.push_back(b);
-  }
+  for (int i = 0; i < n; ++i) v.push_back(single_btimes_item(Y[i], nb, M + (size_t)i * nb * nb, nb, out[i], kbs[i]->n_pw, alpha, beta));
   exec.btimes_batch(v);
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
 }
@@ -2045,7 +1827,7 @@ int lobpcg_run_slab(dftk_b200_kblock* kb, cplx* Xfull, int64_t M, double tol, in
   L.prepare(A);
   // the slab of X lives behind the solver's workspace
   cplx* Xloc = kb->slab_x.ensure((size_t)L.N * M);
-  LAUNCH(ctx, k_copy2d, nblk(L.N * M), 256, 0, Xloc, L.N, (const cplx*)(Xfull + L.row0), Nf, L.N, M);
+  L.copy2d(Mat{Xloc, L.N, L.N, M}, Mat{Xfull + L.row0, Nf, L.N, M});
   A.X = Xloc;
   L.body(A);
   // reassemble: the staging area (Nfull x ceil(M/R) x 3 complex numbers behind the workspace) takes one rank's slab at a time
@@ -2055,7 +1837,7 @@ int lobpcg_run_slab(dftk_b200_kblock* kb, cplx* Xfull, int64_t M, double tol, in
   for (int r = 0; r < R; ++r) {
     const int64_t nr = L.row_off[r + 1] - L.row_off[r];
     NCCL_CHECK(ncclBroadcast(Xloc, stage, (size_t)(2 * nr * M), ncclFloat64, r, ctx->nccl, ctx->stream));
-    LAUNCH(ctx, k_copy2d, nblk(nr * M), 256, 0, Xfull + L.row_off[r], Nf, (const cplx*)stage, nr, nr, M);
+    L.copy2d(Mat{Xfull + L.row_off[r], Nf, nr, M}, Mat{stage, nr, nr, M});
   }
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
   if (exchange_bytes) *exchange_bytes = (double)L.slab_exchange_bytes;

@@ -1,8 +1,9 @@
 // Batched kernels of the small-matrix LOBPCG path: every launch serves one operation of MANY independent (k, spin)
 // blocks (blockIdx.y = item), so that the 29-84 small eigenproblems of BASELINE configs C1/C2/C4/C5 share launches
 // and host synchronisations instead of paying them one k-block at a time (reference seam: the independent per-k solves
-// of src/eigen/diag.jl:16-52).  The per-item work is exactly the single-problem kernel body (lobpcg_small.cuh and the
-// elementwise kernels of lobpcg.cu); item descriptors live in a device-side ring that the host fills per launch.
+// of src/eigen/diag.jl:16-52).  The per-item work is the single-problem body: lobpcg_small.cuh for the small dense
+// algebra, item_body below for the elementwise and reduction operations, which the direct solver path launches for one
+// item through k_item.  Item descriptors live in a device-side ring that the host fills per launch.
 #pragma once
 #include "lobpcg_small.cuh"
 
@@ -21,9 +22,9 @@ struct CholItem { const cplx* O; long long ldo; int n; cplx* invR; long long ldi
 struct RmulItem { cplx* X; long long ld, n_rows; int n; const cplx* invR; long long ldr; };
 struct BtimesItem { SmallMatList Y; const cplx* cm; long long ldcm; int ncols; cplx* out; long long ldo, n_rows; double alpha, beta; };
 struct HeevItem { cplx* G; long long ldg; int n; double* w; cplx* V; double* stats; double* lam_out; int n_keep; };
-struct ResidualItem { const cplx* AX; const cplx* X; const double* lam; cplx* R; long long ld, n_rows; int n_cols; const double* kin; double* norms; double* meankin; };
+struct ResidualItem { const cplx* AX; const cplx* X; const double* lam; cplx* R; long long ld, n_rows; int n_cols, squared; const double* kin; double* norms; double* meankin; };
 struct PrecondItem { cplx* R; long long ld, n_rows; int n_cols; const double* kin; const double* meankin; };
-struct ColnormItem { const cplx* X; long long ld, n_rows; int n_cols; double* norms; };
+struct ColnormItem { const cplx* X; long long ld, n_rows; int n_cols, squared; double* norms; };
 struct ScaleItem { cplx* X; long long ld, n_rows; int n_cols; const double* norms; };
 struct Copy2dItem { cplx* dst; long long ldd; const cplx* src; long long lds, n_rows; int n_cols; };   // src == nullptr: zero fill
 struct MakecpItem { cplx* cP; const cplx* cX; long long ld; int n_rows, n_cols, c0, lenXn; };
@@ -115,30 +116,6 @@ __device__ __forceinline__ void block_sum2(double& a, double& b) {
   }
 }
 
-// R = AX - X lam; norms = ||R||; meankin = <X|kin|X>  (one CTA per column; lobpcg_hyper_impl.jl:443-445 + precondprep!)
-__global__ void __launch_bounds__(256) kb_residual(const ResidualItem* __restrict__ items) {
-  const ResidualItem it = items[blockIdx.y];
-  const int col = blockIdx.x;
-  if (col >= it.n_cols) return;
-  const cplx* ax = it.AX + it.ld * col;
-  const cplx* x = it.X + it.ld * col;
-  cplx* r = it.R + it.ld * col;
-  const double l = it.lam[col];
-  double s = 0.0, mk = 0.0;
-  for (long long i = threadIdx.x; i < it.n_rows; i += blockDim.x) {
-    const cplx a = ax[i], b = x[i];
-    const cplx v = make_double2(a.x - l * b.x, a.y - l * b.y);
-    r[i] = v;
-    s += v.x * v.x + v.y * v.y;
-    if (it.kin) mk += it.kin[i] * (b.x * b.x + b.y * b.y);
-  }
-  block_sum2(s, mk);
-  if (threadIdx.x == 0) {
-    it.norms[col] = sqrt(s);
-    it.meankin[col] = mk;
-  }
-}
-
 // compute_λ of the start vectors: lam = real(<x|Ax> / <x|x>)   (lobpcg_hyper_impl.jl:341-344)
 __global__ void __launch_bounds__(256) kb_lambda(const LambdaItem* __restrict__ items) {
   const LambdaItem it = items[blockIdx.y];
@@ -159,8 +136,37 @@ __global__ void __launch_bounds__(256) kb_lambda(const LambdaItem* __restrict__ 
   if (threadIdx.x == 0) it.lam[col] = nre / d;    // <x|x> is real: the complex division keeps the real part only
 }
 
-__global__ void __launch_bounds__(256) kb_precondition(const PrecondItem* __restrict__ items) {
-  const PrecondItem it = items[blockIdx.y];
+// ---- The block operations shared by both solver paths.  Each has ONE per-item body, run by two entry shapes: the batched
+//      kb_* kernel (items[blockIdx.y], or items[blockIdx.x] for one-CTA items, from the descriptor ring) and k_item (a single
+//      item passed by value as the kernel parameter: the direct path, no descriptor upload).  The elementwise bodies loop
+//      with a grid stride; a direct launch of one thread per element runs one iteration per thread.
+
+// R = AX - X lam; norms = ||R||; meankin = <X|kin|X>  (one CTA per column; lobpcg_hyper_impl.jl:443-445 + precondprep!)
+// squared: norms = ||R||^2 of this rank's rows (slab solves: summed over the ranks, then square-rooted)
+__device__ __forceinline__ void item_body(const ResidualItem& it) {
+  const int col = blockIdx.x;
+  if (col >= it.n_cols) return;
+  const cplx* ax = it.AX + it.ld * col;
+  const cplx* x = it.X + it.ld * col;
+  cplx* r = it.R + it.ld * col;
+  const double l = it.lam[col];
+  double s = 0.0, mk = 0.0;
+  for (long long i = threadIdx.x; i < it.n_rows; i += blockDim.x) {
+    const cplx a = ax[i], b = x[i];
+    const cplx v = make_double2(a.x - l * b.x, a.y - l * b.y);
+    r[i] = v;
+    s += v.x * v.x + v.y * v.y;
+    if (it.kin) mk += it.kin[i] * (b.x * b.x + b.y * b.y);
+  }
+  block_sum2(s, mk);
+  if (threadIdx.x == 0) {
+    it.norms[col] = it.squared ? s : sqrt(s);
+    it.meankin[col] = mk;
+  }
+}
+
+// R[:,n] *= mk_n / (mk_n + kin)    (ldiv!(::PreconditionerTPA), src/gpu/linalg.jl:29-36)
+__device__ __forceinline__ void item_body(const PrecondItem& it) {
   const long long total = it.n_rows * it.n_cols;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const long long i = idx % it.n_rows, c = idx / it.n_rows;
@@ -171,8 +177,8 @@ __global__ void __launch_bounds__(256) kb_precondition(const PrecondItem* __rest
   }
 }
 
-__global__ void __launch_bounds__(256) kb_col_norms(const ColnormItem* __restrict__ items) {
-  const ColnormItem it = items[blockIdx.y];
+// norms = ||X[:,n]|| (||X[:,n]||^2 when `squared`, as for the residual); one CTA per column
+__device__ __forceinline__ void item_body(const ColnormItem& it) {
   const int col = blockIdx.x;
   if (col >= it.n_cols) return;
   const cplx* x = it.X + it.ld * col;
@@ -182,11 +188,10 @@ __global__ void __launch_bounds__(256) kb_col_norms(const ColnormItem* __restric
     s += v.x * v.x + v.y * v.y;
   }
   block_sum2(s, z);
-  if (threadIdx.x == 0) it.norms[col] = sqrt(s);
+  if (threadIdx.x == 0) it.norms[col] = it.squared ? s : sqrt(s);
 }
 
-__global__ void __launch_bounds__(256) kb_scale_cols_inv(const ScaleItem* __restrict__ items) {
-  const ScaleItem it = items[blockIdx.y];
+__device__ __forceinline__ void item_body(const ScaleItem& it) {
   const long long total = it.n_rows * it.n_cols;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const long long i = idx % it.n_rows, c = idx / it.n_rows;
@@ -196,8 +201,8 @@ __global__ void __launch_bounds__(256) kb_scale_cols_inv(const ScaleItem* __rest
   }
 }
 
-__global__ void __launch_bounds__(256) kb_copy2d(const Copy2dItem* __restrict__ items) {
-  const Copy2dItem it = items[blockIdx.y];
+// strided 2D copy (dst and src column-major with different leading dimensions)
+__device__ __forceinline__ void item_body(const Copy2dItem& it) {
   const long long total = it.n_rows * it.n_cols;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const long long i = idx % it.n_rows, c = idx / it.n_rows;
@@ -205,9 +210,8 @@ __global__ void __launch_bounds__(256) kb_copy2d(const Copy2dItem* __restrict__ 
   }
 }
 
-// cP = cX[:, c0:] - e   (lobpcg_hyper_impl.jl:495-503)
-__global__ void __launch_bounds__(256) kb_make_cP(const MakecpItem* __restrict__ items) {
-  const MakecpItem it = items[blockIdx.y];
+// cP = cX[:, c0:] - e,  e[c0 + c, c] = 1 for c < lenXn   (lobpcg_hyper_impl.jl:495-503)
+__device__ __forceinline__ void item_body(const MakecpItem& it) {
   const int total = it.n_rows * it.n_cols;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
     const int i = idx % it.n_rows, c = idx / it.n_rows;
@@ -218,9 +222,8 @@ __global__ void __launch_bounds__(256) kb_make_cP(const MakecpItem* __restrict__
   }
 }
 
-// stats[0] = max |diag|, stats[1] = sum |offdiag|^2, stats[2] = #nan/inf, stats[3] = sum |all|^2   (one CTA per item)
-__global__ void __launch_bounds__(256) kb_matrix_stats(const StatsItem* __restrict__ items) {
-  const StatsItem it = items[blockIdx.x];
+// stats[0] = max |diag|, stats[1] = sum |offdiag|^2, stats[2] = #nan/inf, stats[3] = sum |all|^2   (one CTA, <= 1024 threads)
+__device__ __forceinline__ void item_body(const StatsItem& it) {
   double md = 0.0, so = 0.0, bad = 0.0, sa = 0.0;
   for (int idx = threadIdx.x; idx < it.n_rows * it.n_cols; idx += blockDim.x) {
     const int i = idx % it.n_rows, j = idx / it.n_rows;
@@ -231,7 +234,7 @@ __global__ void __launch_bounds__(256) kb_matrix_stats(const StatsItem* __restri
     if (i == j) md = fmax(md, sqrt(a2));
     else so += a2;
   }
-  __shared__ double r0[8];
+  __shared__ double r0[32];
   for (int o = 16; o > 0; o >>= 1) md = fmax(md, __shfl_down_sync(0xffffffffu, md, o));
   if ((threadIdx.x & 31) == 0) r0[threadIdx.x >> 5] = md;
   __syncthreads();
@@ -248,21 +251,56 @@ __global__ void __launch_bounds__(256) kb_matrix_stats(const StatsItem* __restri
   }
 }
 
-__device__ __forceinline__ unsigned long long batch_splitmix(unsigned long long x) {
+// counter-based normal random numbers (random start vectors, drop_small!'s re-randomisation; statistically plain):
+// x[i] from the SplitMix64 finaliser of the counters seed + 2i and seed + 2i + 1
+__device__ __forceinline__ unsigned long long counter_hash(unsigned long long x) {
   x += 0x9E3779B97F4A7C15ull;
   x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
   return x ^ (x >> 31);
 }
-__global__ void __launch_bounds__(256) kb_randn_col(const RandnItem* __restrict__ items) {
-  const RandnItem it = items[blockIdx.y];
+__device__ __forceinline__ void item_body(const RandnItem& it) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < it.n_rows; i += (long long)gridDim.x * blockDim.x) {
-    const unsigned long long a = batch_splitmix(it.seed + 2 * (unsigned long long)i), b = batch_splitmix(it.seed + 2 * (unsigned long long)i + 1);
+    const unsigned long long a = counter_hash(it.seed + 2 * (unsigned long long)i), b = counter_hash(it.seed + 2 * (unsigned long long)i + 1);
     const double u1 = ((a >> 11) + 1.0) * (1.0 / 9007199254740993.0);
     const double u2 = (b >> 11) * (1.0 / 9007199254740992.0);
     const double r = sqrt(-2.0 * log(u1));
     it.x[i] = make_double2(r * cospi(2.0 * u2) * 0.70710678118654752, r * sinpi(2.0 * u2) * 0.70710678118654752);
   }
+}
+
+template <class Item>
+__global__ void k_item(const Item it) { item_body(it); }
+
+// the item is read in place: a copy would hold `squared` in a register through the loop (48 instead of 40 registers)
+__global__ void __launch_bounds__(256) kb_residual(const ResidualItem* __restrict__ items) { item_body(items[blockIdx.y]); }
+__global__ void __launch_bounds__(256) kb_precondition(const PrecondItem* __restrict__ items) {
+  const PrecondItem it = items[blockIdx.y];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_col_norms(const ColnormItem* __restrict__ items) {
+  const ColnormItem it = items[blockIdx.y];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_scale_cols_inv(const ScaleItem* __restrict__ items) {
+  const ScaleItem it = items[blockIdx.y];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_copy2d(const Copy2dItem* __restrict__ items) {
+  const Copy2dItem it = items[blockIdx.y];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_make_cP(const MakecpItem* __restrict__ items) {
+  const MakecpItem it = items[blockIdx.y];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_matrix_stats(const StatsItem* __restrict__ items) {   // one CTA per item
+  const StatsItem it = items[blockIdx.x];
+  item_body(it);
+}
+__global__ void __launch_bounds__(256) kb_randn_col(const RandnItem* __restrict__ items) {
+  const RandnItem it = items[blockIdx.y];
+  item_body(it);
 }
 
 // <x_n|kin|x_n> per band (ene_ops(::TermKinetic), src/terms/kinetic.jl:40-57); one CTA per (band, item)

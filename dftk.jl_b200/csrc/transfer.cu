@@ -82,25 +82,13 @@ void check_dev_ptr(const void* p, const char* what) {
   REQUIRE(p && is_device_ptr(p), std::string(what) + ": arrays must be device memory");
 }
 
-int fail(dftk_b200_ctx* ctx, int code, const char* msg) {
-  if (ctx) ctx->last_error = msg;
-  return code;
-}
-
 }  // namespace
-
-#define TR_BEGIN try {
-#define TR_END(ctx)                                                                   \
-  }                                                                                   \
-  catch (const dftk::Error& e) { return fail((ctx), e.code, e.what()); }              \
-  catch (const std::exception& e) { return fail((ctx), DFTK_B200_EINVAL, e.what()); } \
-  return DFTK_B200_OK;
 
 extern "C" {
 
 int dftk_b200_remap_tables(dftk_b200_ctx* ctx, int64_t n_G, const int64_t* G, const int32_t* M, const int32_t* delta,
                            const double* tau, const int64_t* lookup, int nx, int ny, int nz, int64_t* idx, void* phase) {
-  TR_BEGIN
+  API_BEGIN
   REQUIRE(ctx && n_G >= 0 && M && delta && (tau || !phase), "remap_tables: bad argument");
   check_cube(nx, ny, nz, "remap_tables");
   REQUIRE(!is_device_ptr(M) && !is_device_ptr(delta) && !(tau && is_device_ptr(tau)), "remap_tables: M, delta and tau are host arrays");
@@ -117,13 +105,13 @@ int dftk_b200_remap_tables(dftk_b200_ctx* ctx, int64_t n_G, const int64_t* G, co
   }
   LAUNCH(ctx, k_remap_tables, (unsigned)((n_G + TR_THREADS - 1) / TR_THREADS), TR_THREADS, 0, (long long)n_G,
          (const long long*)G, a, (const long long*)lookup, nx, ny, nz, (long long*)idx, (cplx*)phase);
-  TR_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_sphere_remap(dftk_b200_ctx* ctx, int64_t n_pairs, const void* const* src, const int64_t* ld_src, void* const* dst,
                            const int64_t* ld_dst, const int64_t* row_offset, const int64_t* n_bands,
                            const int64_t* const* idx, const int64_t* n_dst, const void* const* phase) {
-  TR_BEGIN
+  API_BEGIN
   REQUIRE(ctx && n_pairs >= 0, "sphere_remap: bad argument");
   if (n_pairs == 0) return DFTK_B200_OK;
   REQUIRE(src && ld_src && dst && ld_dst && n_bands && idx && n_dst, "sphere_remap: NULL argument list");
@@ -153,12 +141,12 @@ int dftk_b200_sphere_remap(dftk_b200_ctx* ctx, int64_t n_pairs, const void* cons
   REQUIRE(gz <= 65535, "sphere_remap: too many bands");
   LAUNCH(ctx, k_sphere_remap, dim3(gx, (unsigned)items.size(), gz), TR_THREADS, 0, (const TrRemapItem*)d);
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));   // the descriptor vector is released on return
-  TR_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_fourier_block_copy(dftk_b200_ctx* ctx, const void* in, int nx_in, int ny_in, int nz_in, void* out, int nx_out,
                                  int ny_out, int nz_out, int64_t batch) {
-  TR_BEGIN
+  API_BEGIN
   REQUIRE(ctx && batch >= 0 && batch <= 65535, "fourier_block_copy: bad argument");
   check_cube(nx_in, ny_in, nz_in, "fourier_block_copy");
   check_cube(nx_out, ny_out, nz_out, "fourier_block_copy");
@@ -169,22 +157,22 @@ int dftk_b200_fourier_block_copy(dftk_b200_ctx* ctx, const void* in, int nx_in, 
   const long long No = (long long)nx_out * ny_out * nz_out;
   LAUNCH(ctx, k_block_copy, dim3(tr_grid(ctx, No), (unsigned)batch), TR_THREADS, 0, (const cplx*)in, nx_in, ny_in, nz_in,
          (cplx*)out, nx_out, ny_out, nz_out);
-  TR_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_bspline2_prefilter(dftk_b200_ctx* ctx, void* f, int nx, int ny, int nz, int64_t batch) {
-  TR_BEGIN
+  API_BEGIN
   REQUIRE(ctx && batch >= 0, "bspline2_prefilter: bad argument");
   check_cube(nx, ny, nz, "bspline2_prefilter");
   if (batch == 0) return DFTK_B200_OK;
   check_dev_ptr(f, "bspline2_prefilter");
   LAUNCH(ctx, k_bspline_prefilter, tr_grid(ctx, (long long)nx * ny * nz), TR_THREADS, 0, (cplx*)f, nx, ny, nz, (long long)batch);
-  TR_END(ctx)
+  API_END(ctx)
 }
 
 int dftk_b200_bspline2_evaluate(dftk_b200_ctx* ctx, const double* f, int nx, int ny, int nz, const int32_t* rep, double* out,
                                 int nx_out, int ny_out, int nz_out, int64_t batch, int direct) {
-  TR_BEGIN
+  API_BEGIN
   REQUIRE(ctx && rep && batch >= 0 && batch <= 65535, "bspline2_evaluate: bad argument");
   REQUIRE(!is_device_ptr(rep) && rep[0] >= 1 && rep[1] >= 1 && rep[2] >= 1, "bspline2_evaluate: rep must be 3 positive host integers");
   check_cube(nx, ny, nz, "bspline2_evaluate");
@@ -200,7 +188,7 @@ int dftk_b200_bspline2_evaluate(dftk_b200_ctx* ctx, const double* f, int nx, int
   const long long No = (long long)nx_out * ny_out * nz_out;
   LAUNCH(ctx, k_bspline_eval, dim3(tr_grid(ctx, No), (unsigned)batch), TR_THREADS, 0, f, nx, ny, nz, r, out, nx_out, ny_out,
          nz_out, direct);
-  TR_END(ctx)
+  API_END(ctx)
 }
 
 }  // extern "C"
