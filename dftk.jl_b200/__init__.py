@@ -79,3 +79,6 @@ from .scf import (self_consistent_field, next_density, AdaptiveBands, FixedBands
 from .direct_minimization import direct_minimization, select_occupied_orbitals
 from .transfer import (transfer_mapping, transfer_blochwave_kpt, transfer_blochwave, transfer_density, interpolate_density,
                        apply_symop, unfold_bz, create_supercell, cell_to_supercell)
+from .wannier import (GaussianWannierProjection, HydrogenicWannierProjection, default_wannier_centers, overlap_Mmn_k_kpb,
+                      compute_amn_kpoint, write_w90_win, read_w90_nnkp, write_w90_eig, write_w90_unk, write_w90_mmn,
+                      write_w90_amn, write_wannier90_files, run_wannier90)

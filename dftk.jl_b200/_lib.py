@@ -80,6 +80,7 @@ SIGNATURES = {
     "dftk_b200_fourier_block_copy": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_i64]),
     "dftk_b200_bspline2_prefilter": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_i64]),
     "dftk_b200_bspline2_evaluate": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_i64, c_int]),
+    "dftk_b200_overlap_multi": (c_int, [c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
 }
 
 _lib = None

@@ -146,6 +146,9 @@ struct dftk_b200_ctx {
   dftk::DevBuf<double> dm_ws, dm_out, dm_w, dm_stats;
   dftk::DevBuf<dftk::cplx> dm_C, dm_M, dm_V;
   dftk::DevBuf<char> tr_items;   // basis transfers (transfer.cu): descriptors of the pairs of one sphere remap
+  // batched overlap products (overlap.cu): group and pair descriptors, chunk partials, the gathered block of the large path
+  dftk::DevBuf<char> ov_items;
+  dftk::DevBuf<dftk::cplx> ov_ws, ov_scratch;
 };
 
 namespace dftk {

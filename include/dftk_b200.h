@@ -332,6 +332,18 @@ int dftk_b200_bspline2_prefilter(dftk_b200_ctx* ctx, void* f, int nx, int ny, in
  * axis): f holds the samples themselves and out is their periodic tiling.  out: batch x (nx_out ny_out nz_out) real (device). */
 int dftk_b200_bspline2_evaluate(dftk_b200_ctx* ctx, const double* f, int nx, int ny, int nz, const int32_t* rep, double* out,
                                 int nx_out, int ny_out, int nz_out, int64_t batch, int direct);
+/* Batched overlap products with an indirect right operand, one call for all n_pairs pairs (host arrays of n_pairs entries):
+ *   C_p[m, n] = Σ_{j < n_G[p]} conj(A_p[m, j]) · B_p[n, idx_p[j]]   for m < n_a, n < n_b,
+ * idx_p[j] = -1 contributing nothing and a NULL idx (list or entry) meaning idx_p[j] = j.  A_p: n_a rows of length ld_a[p]
+ * (>= n_G[p]), B_p: n_b rows of length ld_b[p], complex128 (device), a band per row; idx_p: n_G[p] int64 (device), in range
+ * [-1, ld_b[p]) by the caller's contract, as for sphere_remap.  C: n_pairs column-major n_a × n_b matrices (device).  The
+ * Wannier90 overlaps M^{k,b} (A = ψ_k, B = ψ_{k+b}, idx from remap_tables with M = I and delta = G_shift) and projections A_k
+ * (B = the projection table of k, idx NULL, src/external/wannier_shared.jl).  Up to 32 columns: a fused gather-product in two
+ * launches whatever the pair count; consecutive pairs with the same A (pointer, ld_a, n_G) read A once; fixed-order sums, so a
+ * rerun is bit-identical.  Larger blocks: per pair a gather into scratch and the DMMA ZGEMM. */
+int dftk_b200_overlap_multi(dftk_b200_ctx* ctx, int64_t n_pairs, int64_t n_a, int64_t n_b, const void* const* A,
+                            const int64_t* ld_a, const int64_t* n_G, const void* const* B, const int64_t* ld_b,
+                            const int64_t* const* idx, void* C);
 
 #ifdef __cplusplus
 }
