@@ -74,7 +74,7 @@ from .forces import (compute_forces, compute_forces_cart, symmetrize_forces, ene
 from .hubbard import (OrbitalManifold, Hubbard, TermHubbard, atomic_orbital_projectors, atomic_orbital_projections,
                       compute_hubbard_n, symmetrize_hubbard_n, wigner_d_matrix, resolve_hubbard_manifold)
 from .scf import (self_consistent_field, next_density, AdaptiveBands, FixedBands, AdaptiveDiagtol,
-                  ScfConvergenceDensity, ScfConvergenceEnergy, SimpleMixing, KerkerMixing, LdosMixing, compute_ldos,
+                  ScfConvergenceDensity, ScfConvergenceEnergy, SimpleMixing, KerkerMixing, LdosMixing,
                   AndersonAcceleration, ScfDefaultCallback)
 from .direct_minimization import direct_minimization, select_occupied_orbitals
 from .transfer import (transfer_mapping, transfer_blochwave_kpt, transfer_blochwave, transfer_density, interpolate_density,
@@ -82,3 +82,4 @@ from .transfer import (transfer_mapping, transfer_blochwave_kpt, transfer_blochw
 from .wannier import (GaussianWannierProjection, HydrogenicWannierProjection, default_wannier_centers, overlap_Mmn_k_kpb,
                       compute_amn_kpoint, write_w90_win, read_w90_nnkp, write_w90_eig, write_w90_unk, write_w90_mmn,
                       write_w90_amn, write_wannier90_files, run_wannier90)
+from .dos import compute_dos, compute_ldos, compute_pdos, sum_pdos, PdosResult

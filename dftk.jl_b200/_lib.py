@@ -49,6 +49,7 @@ SIGNATURES = {
     "dftk_b200_band_energies": (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp]),
     "dftk_b200_band_energies_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "dftk_b200_density_accumulate_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "dftk_b200_ldos_accumulate_multi": (c_int, [c_i64, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp]),
     "dftk_b200_lobpcg": (c_int, [c_vp, c_vp, c_i64, c_dbl, c_int, c_int, c_i64, c_int, c_vp, c_vp,
                                  P(c_int), P(c_i64), P(c_int)]),
     "dftk_b200_lobpcg_slab": (c_int, [c_vp, c_vp, c_i64, c_dbl, c_int, c_int, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -555,6 +555,8 @@ int dftk_b200_kblock_trim(dftk_b200_kblock* kb) {
   }
   kb->W1.release();
   kb->W2.release();
+  kb->ldos_cube.release();
+  kb->ldos_rho.release();
   kb->proj.release();
   kb->fold_ws.release();
   API_END(ctx)

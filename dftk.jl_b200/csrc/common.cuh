@@ -149,6 +149,7 @@ struct dftk_b200_ctx {
   // batched overlap products (overlap.cu): group and pair descriptors, chunk partials, the gathered block of the large path
   dftk::DevBuf<char> ov_items;
   dftk::DevBuf<dftk::cplx> ov_ws, ov_scratch;
+  dftk::DevBuf<char> ldos_items;   // LDOS pass (ldos.cu): the density-row and weight-column pointers of every round
 };
 
 namespace dftk {

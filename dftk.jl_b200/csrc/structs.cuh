@@ -100,6 +100,8 @@ struct dftk_b200_kblock {
   const double* Vtp() const { return grid_V >= 0 ? grid->Vts[grid_V].p : Vt.p; }
   // scratch
   dftk::DevBuf<dftk::cplx> W1, W2;    // pruned intermediates for a chunk of bands
+  dftk::DevBuf<dftk::cplx> ldos_cube; // LDOS pass (ldos.cu): the cubes of a chunk of bands, then their |ψ|²/Ω
+  dftk::DevBuf<double> ldos_rho;
   dftk::DevBuf<dftk::cplx> proj;      // n_proj x n_bands (+ D*proj)
   dftk::DevBuf<dftk::cplx> lobpcg_ws; // big LOBPCG workspace
   dftk::DevBuf<dftk::cplx> small_ws;  // small dense LOBPCG workspace

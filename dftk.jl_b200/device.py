@@ -175,6 +175,23 @@ def density_accumulate_multi(kblocks, psis, weights, rho):
     return rho
 
 
+def ldos_accumulate_multi(kblocks, psis, W, ldos):
+    """dftk_b200_ldos_accumulate_multi: ldos (n_ε, n_spin, N) += Σ_blocks Σ_n W[j, i, n] |IFFT psi_n|² / Ω, each block into the
+    channel of its spin.  psis[i]: (nb_i, n_pw_i) contiguous device tensors, W: (n_ε, n_blocks, ld_w) float64 device tensor;
+    a band whose weight is zero at every energy is skipped."""
+    n = len(kblocks)
+    if n == 0:
+        return ldos
+    ctx = kblocks[0].ctx
+    assert W.is_contiguous() and ldos.is_contiguous() and W.shape[:2] == (ldos.shape[0], n)
+    nbs = np.array([p.shape[0] for p in psis], dtype=np.int32)
+    kb_arr = (c_vp * n)(*[kb.h.value for kb in kblocks])
+    x_arr = (c_vp * n)(*[p.data_ptr() for p in psis])
+    check(ctx.L.dftk_b200_ldos_accumulate_multi(n, kb_arr, x_arr, _ptr(nbs), ldos.shape[0], ldos.shape[1], _ptr(W), W.shape[2],
+                                                _ptr(ldos)), ctx.h)
+    return ldos
+
+
 def orbital_occupation_multi(kblocks, psis, weights, n_spin, n_orb):
     """dftk_b200_orbital_occupation_multi: Σ_blocks Σ_n w_n (Φ'ψ_n)(Φ'ψ_n)' per spin channel over the Hubbard orbitals of
     the k-blocks.  psis[i]: (nb_i, n_pw_i) contiguous device tensors, weights[i]: nb_i host numbers.  Returns a

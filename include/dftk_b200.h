@@ -196,6 +196,17 @@ int dftk_b200_density_accumulate(dftk_b200_kblock* kb, const void* psi, const do
 int dftk_b200_density_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* psi,
                                        const double* occ_w_host, int64_t ld_w, const int32_t* n_bands, double* rho);
 
+/* The LDOS at n_energies energies in one pass over the bands (compute_ldos, src/postprocess/dos.jl):
+ *   ldos[j, σ, :] += Σ_blocks of spin σ Σ_n W[j, i, n] |IFFT psi_n|² / Ω
+ * W (device): n_energies × n_blocks × ld_w doubles, W[(j n_blocks + i) ld_w + n] the weight of band n of block i at energy j
+ * (k-point weight included); ldos (device): n_energies × n_spin × N_fft.  A band whose weight is zero at every energy is
+ * neither transformed nor multiplied.  Each kept band is transformed once with the density pass's sphere -> cube FFT, staged
+ * as |ψ|²/Ω in k-block scratch (released by kblock_trim), and multiplied into all energies by a real FP64 DMMA product;
+ * fixed-order sums, so a rerun is bit-identical.  n_spin is the model's: a rank may hold blocks of one spin only. */
+int dftk_b200_ldos_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const* kblocks, const void* const* psi,
+                                    const int32_t* n_bands, int64_t n_energies, int64_t n_spin, const double* W /*dev*/,
+                                    int64_t ld_w, double* ldos /*dev: n_energies × n_spin × N_fft*/);
+
 /* ---- collectives (mpi_sum!/mpi_min/mpi_max over basis.comm_kpts, src/common/mpi.jl:19-31) ---- */
 int dftk_b200_allreduce(dftk_b200_ctx* ctx, void* buf /*dev*/, int64_t count, int dtype,
                         int op /*0 sum, 1 min, 2 max*/);
