@@ -161,14 +161,8 @@ int dftk_b200_ctx_destroy(dftk_b200_ctx* ctx) {
       cudaEventDestroy(ctx->ev_out[i]);
     }
   }
-  if (ctx->batch_ring_h) cudaFreeHost(ctx->batch_ring_h);
-  if (ctx->batch_gather_h) cudaFreeHost(ctx->batch_gather_h);
-  if (ctx->batch_ring_h2) cudaFreeHost(ctx->batch_ring_h2);
-  if (ctx->batch_gather_h2) cudaFreeHost(ctx->batch_gather_h2);
-  for (int i = 0; i < 2; ++i) {
+  for (int i = 0; i < 2; ++i)
     if (ctx->batch_streams[i]) cudaStreamDestroy(ctx->batch_streams[i]);
-    if (ctx->batch_events[i]) cudaEventDestroy(ctx->batch_events[i]);
-  }
   if (ctx->nccl) ncclCommDestroy(ctx->nccl);
   if (ctx->cublas) cublasDestroy(ctx->cublas);
   if (ctx->solver_params) cusolverDnDestroyParams(ctx->solver_params);
@@ -465,9 +459,11 @@ int dftk_b200_orbital_occupation_multi(int64_t n_blocks, dftk_b200_kblock* const
   REQUIRE(n_blocks >= 0 && (n_blocks == 0 || (kbs && psi && occ_w_host && n_bands && n_out)),
           "orbital_occupation_multi: bad argument");
   if (n_blocks == 0) return DFTK_B200_OK;
-  REQUIRE(is_device_ptr(n_out), "orbital_occupation_multi: n_out must be device memory");
-  for (int64_t i = 0; i < n_blocks; ++i)
-    REQUIRE(kbs[i] && psi[i] && is_device_ptr(psi[i]), "orbital_occupation_multi: orbitals must be device memory");
+  require_device(ctx, n_out, "orbital_occupation_multi: n_out");
+  for (int64_t i = 0; i < n_blocks; ++i) {
+    REQUIRE(kbs[i], "orbital_occupation_multi: NULL k-block");
+    require_device(ctx, psi[i], "orbital_occupation_multi: orbitals");
+  }
   orbital_occupation_multi(n_blocks, kbs, (const cplx* const*)psi, occ_w_host, ld_w, (const int*)n_bands, (cplx*)n_out);
   API_END(ctx)
 }
@@ -679,8 +675,10 @@ int dftk_b200_band_energies_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs
   dftk_b200_ctx* ctx = (n_blocks > 0 && kbs && kbs[0]) ? kbs[0]->grid->ctx : nullptr;
   API_BEGIN
   REQUIRE(n_blocks >= 0 && (n_blocks == 0 || (kbs && psi && n_bands)), "band_energies_multi: bad argument");
-  for (int64_t i = 0; i < n_blocks; ++i)
-    REQUIRE(kbs[i] && psi[i] && is_device_ptr(psi[i]), "band_energies_multi: orbitals must be device memory");
+  for (int64_t i = 0; i < n_blocks; ++i) {
+    REQUIRE(kbs[i], "band_energies_multi: NULL k-block");
+    require_device(ctx, psi[i], "band_energies_multi: orbitals");
+  }
   band_energies_multi(n_blocks, kbs, (const cplx* const*)psi, (const int*)n_bands, ld_out, ekin_host, enl_host);
   API_END(ctx)
 }
@@ -691,10 +689,11 @@ int dftk_b200_density_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const
   API_BEGIN
   REQUIRE(n_blocks >= 0 && (n_blocks == 0 || (kbs && psi && n_bands && occ_w_host && rho)), "density_accumulate_multi: bad argument");
   if (n_blocks == 0) return DFTK_B200_OK;
-  REQUIRE(is_device_ptr(rho), "density_accumulate_multi: rho must be device memory");
-  for (int64_t i = 0; i < n_blocks; ++i)
-    REQUIRE(kbs[i] && psi[i] && is_device_ptr(psi[i]) && n_bands[i] >= 0 && n_bands[i] <= ld_w,
-            "density_accumulate_multi: bad block / orbitals must be device memory");
+  require_device(ctx, rho, "density_accumulate_multi: rho");
+  for (int64_t i = 0; i < n_blocks; ++i) {
+    REQUIRE(kbs[i] && n_bands[i] >= 0 && n_bands[i] <= ld_w, "density_accumulate_multi: bad block");
+    require_device(ctx, psi[i], "density_accumulate_multi: orbitals");
+  }
   if (!kb_density_accumulate_multi((int)n_blocks, kbs, (const cplx* const*)psi, occ_w_host, ld_w, (const int*)n_bands, rho))
     for (int64_t i = 0; i < n_blocks; ++i)       // blocks that do not qualify for the batched kernels: one after the other
       if (n_bands[i] > 0)
@@ -733,8 +732,10 @@ int dftk_b200_lobpcg_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, void*
   if (n_blocks == 0) return DFTK_B200_OK;
   REQUIRE(kbs && X && lambda_host && resid_host && n_iter && n_matvec && converged, "lobpcg_multi: NULL argument");
   REQUIRE(maxiter >= 0 && miniter >= 0, "lobpcg_multi: bad iteration limits");
-  for (int64_t i = 0; i < n_blocks; ++i)
-    REQUIRE(kbs[i] && X[i] && is_device_ptr(X[i]), "lobpcg_multi: orbitals must be device memory");
+  for (int64_t i = 0; i < n_blocks; ++i) {
+    REQUIRE(kbs[i], "lobpcg_multi: NULL k-block");
+    require_device(ctx, X[i], "lobpcg_multi: orbitals");
+  }
   lobpcg_run_multi(n_blocks, kbs, (cplx* const*)X, n_bands, tol, miniter, maxiter, n_conv_check, use_tpa_preconditioner != 0,
                    lambda_host, resid_host, n_iter, n_matvec, converged);
   API_END(ctx)
@@ -757,8 +758,10 @@ int dftk_b200_random_orbitals(int64_t n_blocks, dftk_b200_kblock* const* kbs, vo
   dftk_b200_ctx* ctx = (n_blocks > 0 && kbs && kbs[0]) ? kbs[0]->grid->ctx : nullptr;
   API_BEGIN
   REQUIRE(n_blocks >= 0 && (n_blocks == 0 || (kbs && X)) && n_bands >= 1, "random_orbitals: bad argument");
-  for (int64_t i = 0; i < n_blocks; ++i)
-    REQUIRE(kbs[i] && X[i] && is_device_ptr(X[i]), "random_orbitals: orbitals must be device memory");
+  for (int64_t i = 0; i < n_blocks; ++i) {
+    REQUIRE(kbs[i], "random_orbitals: NULL k-block");
+    require_device(ctx, X[i], "random_orbitals: orbitals");
+  }
   random_orbitals_multi(n_blocks, kbs, (cplx* const*)X, n_bands, seed);
   API_END(ctx)
 }

@@ -10,7 +10,7 @@ SOURCES = ["fft.cu", "blas.cu", "lobpcg.cu", "api.cu", "xc.cu", "forces.cu", "se
 REG_NGROUPS = 4
 HEADERS = ["common.cuh", "structs.cuh", "fft_core.cuh", "fft_plan.h", "fft_reg.cuh", "fft_reg_fwd.cuh", "fft_reg.cu",
            "fft_radix_gen.cuh", "xc_core.cuh", "forces_core.cuh", "lobpcg_small.cuh", "lobpcg_batch.cuh", "i8emu_core.cuh", "dm_core.cuh", "transfer_core.cuh",
-           "overlap_core.cuh", "ldos_core.cuh",
+           "overlap_core.cuh", "ldos_core.cuh", "batch_exec.cuh",
            os.path.join("..", "..", "include", "dftk_b200.h")]
 LIB = os.path.join(HERE, "..", "libdftk_b200.so")
 

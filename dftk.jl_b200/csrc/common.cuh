@@ -5,6 +5,7 @@
 #include <cusolverDn.h>
 #include <nccl.h>
 #include <stdint.h>
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
@@ -78,6 +79,76 @@ struct DevBuf {
   }
 };
 
+// Descriptor ring: the launch data a call builds on the host (item structs, pointer lists, band weights) is copied into a
+// pinned block and from there, in stream order, into a device block of the same size.  The rules that keep a descriptor
+// intact until the kernels reading it have run:
+//  - put() returns the device copy; it stays valid until the next rewind().
+//  - rewind() is called only right after a synchronisation of the stream the puts went to (the end of a scheduler round,
+//    the trailing synchronisation of a one-shot call).
+//  - a put that does not fit behind the data already staged synchronises the stream, then rewinds;
+//  - a put larger than the whole ring synchronises and grows the ring to fit (a put never fails for size);
+//  - a call that puts several regions before the launches that read them first calls reserve() with their total (padded()
+//    each), so that none of its puts wraps over an earlier one.
+// Both blocks are created at first use (cudaMallocHost costs about a millisecond) and kept for the context's lifetime.
+struct DescRing {
+  char* host = nullptr;
+  DevBuf<char> dev;
+  size_t cap = 0, off = 0;
+  ~DescRing() {
+    if (host) cudaFreeHost(host);
+  }
+  static size_t padded(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+  template <class T>
+  static size_t padded(const std::vector<T>& v) { return padded(v.size() * sizeof(T)); }
+  void reserve(size_t bytes, cudaStream_t s) {
+    bytes = padded(bytes);
+    if (off + bytes <= cap) return;
+    if (cap) CUDA_CHECK(cudaStreamSynchronize(s));
+    off = 0;
+    if (bytes <= cap) return;
+    if (host) CUDA_CHECK(cudaFreeHost(host));
+    host = nullptr;
+    cap = 0;
+    const size_t n = std::max(bytes, (size_t)4 << 20);
+    CUDA_CHECK(cudaMallocHost((void**)&host, n));
+    dev.ensure(n);
+    cap = n;
+  }
+  const void* put(const void* src, size_t bytes, cudaStream_t s) {
+    reserve(bytes, s);
+    char* d = dev.p + off;
+    if (bytes) {
+      memcpy(host + off, src, bytes);
+      CUDA_CHECK(cudaMemcpyAsync(d, host + off, bytes, cudaMemcpyHostToDevice, s));
+    }
+    off += padded(bytes);
+    return d;
+  }
+  template <class T>
+  const T* put(const std::vector<T>& v, cudaStream_t s) {
+    return (const T*)put(v.data(), v.size() * sizeof(T), s);
+  }
+  void rewind() { off = 0; }
+};
+
+// One executor slot of the batched small-matrix kernels (BatchExec, lobpcg.cu); slot 1 serves the second group of the
+// pipelined scheduler, slot 0 everything else, including the descriptors of the one-shot multi-block calls.
+struct BatchSlot {
+  static constexpr size_t GATHER_CAP = (size_t)1 << 18;   // doubles of the per-round result gather
+  DescRing ring;
+  DevBuf<double> gather;
+  double* gather_h = nullptr;    // pinned landing zone of the gather
+  DevBuf<char> own_ws;
+  DevBuf<char>* gram_ws;         // per-CTA partials of kb_gram: slot 0 shares the split-K workspace of the GEMMs
+  DevBuf<int> counter;           // arrival counters of kb_gram (kept at zero between launches)
+  cudaEvent_t ev = nullptr;      // end of the issued round
+  explicit BatchSlot(DevBuf<char>* ws = nullptr) : gram_ws(ws ? ws : &own_ws) {}
+  ~BatchSlot() {
+    if (gather_h) cudaFreeHost(gather_h);
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+
 }  // namespace dftk
 
 struct dftk_b200_ctx {
@@ -103,7 +174,6 @@ struct dftk_b200_ctx {
   int z_pipeline = 0;     // fused z stage of the H apply: 0 = one tile per CTA (default), 1 = persistent cp.async-pipelined kernel
   int force_svd_fallback = 0;   // test hook: the next N ortho! calls behave as if safe_cholesky had given up
   int small_dense = 1;    // LOBPCG with <= 32 bands: fused small-matrix kernels (lobpcg_small.cuh); 0 = GEMM + cuSOLVER path
-  dftk::DevBuf<int> small_counter;   // arrival counter of k_small_gram (kept at zero between launches)
   int sm_count = 132;
   int smem_optin = 227 * 1024;   // largest dynamic shared memory of one CTA (cudaDevAttrMaxSharedMemoryPerBlockOptin)
   std::string last_error;
@@ -119,37 +189,23 @@ struct dftk_b200_ctx {
   cudaStream_t s_in = nullptr, s_out = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
   dftk::DevBuf<char> pipe_in[2], pipe_out[2];
-  // batched small-matrix LOBPCG (lobpcg.cu): descriptor ring and per-round result gather, device + pinned host sides
-  dftk::DevBuf<char> batch_ring;
-  dftk::DevBuf<double> batch_gather;
-  char* batch_ring_h = nullptr;
-  double* batch_gather_h = nullptr;
   dftk::DevBuf<signed char> i8_tmp_planes;   // gemm_backend 4: planes of an operand prepared inside a generic zgemm call
   dftk::DevBuf<int> i8_tmp_exps;
-  // second executor of the pipelined batched solves (two groups of k-blocks on two streams: while one group's round runs on
-  // the GPU, the host records and issues the other group's): its own descriptor ring, gather buffer, Gram workspace, counters
-  dftk::DevBuf<char> batch_ring2, batch_ws2;
-  dftk::DevBuf<double> batch_gather2;
-  dftk::DevBuf<int> small_counter2;
-  char* batch_ring_h2 = nullptr;
-  double* batch_gather_h2 = nullptr;
+  // executor slots of the batched small-matrix kernels: slot 1 is the second group of the pipelined batched solves (two
+  // groups of k-blocks on two streams: while one group's round runs on the GPU, the host records and issues the other's)
+  dftk::BatchSlot slot[2]{dftk::BatchSlot(&gemm_ws), dftk::BatchSlot()};
   cudaStream_t batch_streams[2] = {nullptr, nullptr};
-  cudaEvent_t batch_events[2] = {nullptr, nullptr};
   cudaStream_t batch_user_stream = nullptr;   // the context's own stream while a pipelined batch has swapped ctx->stream
   bool batch_pipelined = false;
   int batch_pipeline = 0;     // option: 1 = two pipelined groups for batches of >= 8 k-blocks, 0 (default) = one group (one sync per
                               // round)
   double lobpcg_flops = 0.0;  // FP64-equivalent GEMM flops executed by the large-path LOBPCG solves (Gram, update, Cholesky-QR, nonlocal) since reset
   int64_t batch_rounds = 0;   // scheduler rounds (= host synchronisations) of the batched solves since creation / reset
-  // direct minimisation (dm.cu): item descriptors, reduction partials and results, small matrices of all blocks
-  dftk::DevBuf<char> dm_items;
+  // direct minimisation (dm.cu): reduction partials and results, small matrices of all blocks
   dftk::DevBuf<double> dm_ws, dm_out, dm_w, dm_stats;
   dftk::DevBuf<dftk::cplx> dm_C, dm_M, dm_V;
-  dftk::DevBuf<char> tr_items;   // basis transfers (transfer.cu): descriptors of the pairs of one sphere remap
-  // batched overlap products (overlap.cu): group and pair descriptors, chunk partials, the gathered block of the large path
-  dftk::DevBuf<char> ov_items;
+  // batched overlap products (overlap.cu): chunk partials, the gathered block of the large path
   dftk::DevBuf<dftk::cplx> ov_ws, ov_scratch;
-  dftk::DevBuf<char> ldos_items;   // LDOS pass (ldos.cu): the density-row and weight-column pointers of every round
 };
 
 namespace dftk {
@@ -179,5 +235,13 @@ inline bool is_device_ptr(const void* p) {
     return false;
   }
   return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+// `p` is device or managed memory, and device memory of the context's device; what: "<entry point>: <argument>"
+inline void require_device(const dftk_b200_ctx* ctx, const void* p, const std::string& what) {
+  cudaPointerAttributes a;
+  const cudaError_t e = p ? cudaPointerGetAttributes(&a, p) : cudaErrorInvalidValue;
+  if (e != cudaSuccess) cudaGetLastError();
+  REQUIRE(e == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged), what + " must be device memory");
+  REQUIRE(a.type != cudaMemoryTypeDevice || a.device == ctx->device, what + " must be on the context's device");
 }
 }  // namespace dftk

@@ -4,8 +4,7 @@
 // the block count); larger blocks take the DMMA ZGEMMs and cuSOLVER, one block after the other.
 #include <algorithm>
 #include <cmath>
-#include "structs.cuh"
-#include "lobpcg_small.cuh"
+#include "batch_exec.cuh"
 #include "dm_core.cuh"
 
 using namespace dftk;
@@ -79,12 +78,10 @@ unsigned grid_for(dftk_b200_ctx* ctx, long long total) {
   return (unsigned)std::max<long long>(1, std::min<long long>(g, (long long)ctx->sm_count * 16));
 }
 
-// descriptors go to the device through a buffer of their own, in stream order
-template <class T>
-const T* put(dftk_b200_ctx* ctx, DevBuf<char>& buf, const std::vector<T>& v) {
-  buf.ensure(v.size() * sizeof(T));
-  CUDA_CHECK(cudaMemcpyAsync(buf.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return (const T*)buf.p;
+// the stream synchronisation every entry point ends with; the descriptors it staged are then no longer read
+void finish(dftk_b200_ctx* ctx) {
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ctx->slot[0].ring.rewind();
 }
 
 // Sum_pairs of Re<A, B> (or the fused update + dot) over all block items: two launches, one synchronisation.
@@ -94,13 +91,13 @@ void dots(dftk_b200_ctx* ctx, const std::vector<DmDotItem>& items, int n_pairs, 
   const int n_chunks = (int)std::min<long long>(DM_MAX_CHUNKS, (max_len + DM_THREADS - 1) / DM_THREADS);
   double* ws = ctx->dm_ws.ensure((size_t)items.size() * n_chunks);
   double* out = ctx->dm_out.ensure(std::max(n_pairs, 1));
-  LAUNCH(ctx, k_dm_dot_partial, dim3((unsigned)n_chunks, (unsigned)items.size()), DM_THREADS, 0, put(ctx, ctx->dm_items, items),
-         n_chunks, ws);
+  LAUNCH(ctx, k_dm_dot_partial, dim3((unsigned)n_chunks, (unsigned)items.size()), DM_THREADS, 0,
+         ctx->slot[0].ring.put(items, ctx->stream), n_chunks, ws);
   if (n_pairs > 0) {
     LAUNCH(ctx, k_dm_dot_final, (unsigned)((n_pairs + 63) / 64), 64, 0, (const double*)ws, n_pairs, n_blocks, n_chunks, out);
     CUDA_CHECK(cudaMemcpyAsync(out_host, out, n_pairs * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   }
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  finish(ctx);
 }
 
 void heev_large(dftk_b200_ctx* ctx, cplx* A, int64_t n, double* w) {
@@ -123,7 +120,11 @@ void heev_large(dftk_b200_ctx* ctx, cplx* A, int64_t n, double* w) {
 // C_i = A_i^H B_i (nb x nb at C + i nb^2) for all blocks
 void grams(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* A, const cplx* const* Bm, int nb, cplx* C) {
   if (nb <= SMALL_MAX_N) {
-    dm_small_gram(ctx, n, kbs, A, Bm, nb, C);
+    std::vector<GramItem> v;
+    for (int i = 0; i < n; ++i)
+      v.push_back(single_gram_item(ctx, A[i], kbs[i]->n_pw, nb, Bm[i], kbs[i]->n_pw, nb, kbs[i]->n_pw, C + (size_t)i * nb * nb));
+    BatchExec(ctx, ctx->slot[0]).gram_batch(v);
+    finish(ctx);
     return;
   }
   for (int i = 0; i < n; ++i)
@@ -134,7 +135,11 @@ void grams(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* 
 void times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* Y, const cplx* M, int nb, cplx* const* out,
            double alpha, double beta) {
   if (nb <= SMALL_MAX_N) {
-    dm_small_times(ctx, n, kbs, Y, M, nb, out, alpha, beta);
+    std::vector<BtimesItem> v;
+    for (int i = 0; i < n; ++i)
+      v.push_back(single_btimes_item(Y[i], nb, M + (size_t)i * nb * nb, nb, out[i], kbs[i]->n_pw, alpha, beta));
+    BatchExec(ctx, ctx->slot[0]).btimes_batch(v);
+    finish(ctx);
     return;
   }
   for (int i = 0; i < n; ++i)
@@ -149,9 +154,9 @@ void check_blocks(dftk_b200_ctx* ctx, int64_t n, dftk_b200_kblock* const* kbs, i
   for (int64_t i = 0; i < n; ++i)
     REQUIRE(kbs[i] && kbs[i]->grid->ctx == ctx, std::string(what) + ": all blocks must belong to one context");
 }
-void check_dev(int64_t n, const void* const* p, const char* what) {
+void check_orbitals(dftk_b200_ctx* ctx, int64_t n, const void* const* p, const char* what) {
   REQUIRE(p, std::string(what) + ": NULL block list");
-  for (int64_t i = 0; i < n; ++i) REQUIRE(p[i] && is_device_ptr(p[i]), std::string(what) + ": orbitals must be device memory");
+  for (int64_t i = 0; i < n; ++i) require_device(ctx, p[i], std::string(what) + ": orbitals");
 }
 
 }  // namespace
@@ -164,9 +169,12 @@ int dftk_b200_apply_h_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, cons
   API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "apply_h_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
-  check_dev(n_blocks, psi, "apply_h_multi");
-  check_dev(n_blocks, (const void* const*)out, "apply_h_multi");
-  dm_apply_h(ctx, (int)n_blocks, kbs, (const cplx* const*)psi, (cplx* const*)out, (int)n_bands);
+  check_orbitals(ctx, n_blocks, psi, "apply_h_multi");
+  check_orbitals(ctx, n_blocks, (const void* const*)out, "apply_h_multi");
+  std::vector<ApplyHItem> items;
+  for (int64_t i = 0; i < n_blocks; ++i) items.push_back(ApplyHItem{kbs[i], (const cplx*)psi[i], (cplx*)out[i], (int)n_bands});
+  BatchExec(ctx, ctx->slot[0]).apply_h_batch(items);
+  finish(ctx);
   if (scale_host) {
     std::vector<DmScaleItem> v;
     long long mt = 1;
@@ -174,8 +182,8 @@ int dftk_b200_apply_h_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, cons
       v.push_back(DmScaleItem{(cplx*)out[i], (long long)kbs[i]->n_pw * n_bands, scale_host[i]});
       mt = std::max(mt, v.back().len);
     }
-    LAUNCH(ctx, k_dm_scale, dim3(grid_for(ctx, mt), (unsigned)n_blocks), DM_THREADS, 0, put(ctx, ctx->dm_items, v));
-    CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    LAUNCH(ctx, k_dm_scale, dim3(grid_for(ctx, mt), (unsigned)n_blocks), DM_THREADS, 0, ctx->slot[0].ring.put(v, ctx->stream));
+    finish(ctx);
   }
   API_END(ctx)
 }
@@ -186,8 +194,8 @@ int dftk_b200_stiefel_project_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "stiefel_project_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
-  check_dev(n_blocks, X, "stiefel_project_multi");
-  check_dev(n_blocks, (const void* const*)G, "stiefel_project_multi");
+  check_orbitals(ctx, n_blocks, X, "stiefel_project_multi");
+  check_orbitals(ctx, n_blocks, (const void* const*)G, "stiefel_project_multi");
   const int nb = (int)n_bands, n = (int)n_blocks;
   cplx* C = ctx->dm_C.ensure((size_t)n * nb * nb);
   cplx* M = ctx->dm_M.ensure((size_t)n * nb * nb);
@@ -204,8 +212,8 @@ int dftk_b200_stiefel_retract_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "stiefel_retract_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
-  check_dev(n_blocks, Y, "stiefel_retract_multi");
-  check_dev(n_blocks, (const void* const*)X_out, "stiefel_retract_multi");
+  check_orbitals(ctx, n_blocks, Y, "stiefel_retract_multi");
+  check_orbitals(ctx, n_blocks, (const void* const*)X_out, "stiefel_retract_multi");
   for (int64_t i = 0; i < n_blocks; ++i) REQUIRE(Y[i] != X_out[i], "stiefel_retract_multi: the output must not alias the input");
   const int nb = (int)n_bands, n = (int)n_blocks;
   cplx* C = ctx->dm_C.ensure((size_t)n * nb * nb);
@@ -216,7 +224,11 @@ int dftk_b200_stiefel_retract_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   std::vector<double> w_h((size_t)n * nb);
   if (nb <= SMALL_MAX_N) {
     double* st = ctx->dm_stats.ensure((size_t)2 * n);
-    dm_small_heev(ctx, n, C, nb, w, V, st);                                             // eigenvectors overwrite C
+    std::vector<HeevItem> v;                                                            // eigenvectors overwrite C
+    for (int i = 0; i < n; ++i)
+      v.push_back(HeevItem{C + (size_t)i * nb * nb, nb, nb, w + (size_t)i * nb, V + (size_t)i * nb * nb, st + 2 * i, nullptr, 0});
+    BatchExec(ctx, ctx->slot[0]).heev_batch(v);
+    finish(ctx);
     std::vector<double> st_h((size_t)2 * n);
     CUDA_CHECK(cudaMemcpy(st_h.data(), st, st_h.size() * sizeof(double), cudaMemcpyDeviceToHost));
     for (int i = 0; i < n; ++i)
@@ -251,17 +263,21 @@ int dftk_b200_tpa_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const vo
   API_BEGIN
   check_blocks(ctx, n_blocks, kbs, n_bands, "tpa_multi");
   if (n_blocks == 0) return DFTK_B200_OK;
-  REQUIRE(!use_tpa || (mean_kin && is_device_ptr(mean_kin)), "tpa_multi: mean_kin must be device memory");
+  if (use_tpa) require_device(ctx, mean_kin, "tpa_multi: mean_kin");
   const int n = (int)n_blocks, nb = (int)n_bands;
   if (use_tpa)
     for (int i = 0; i < n; ++i) REQUIRE(kbs[i]->has_kin, "tpa_multi: the TPA preconditioner needs a kinetic term");
   if (X && use_tpa) {     // precondprep!: mean_kin[n] = sum_G kin_G |x_Gn|^2
-    check_dev(n_blocks, X, "tpa_multi");
-    dm_kin_dots(ctx, n, kbs, (const cplx* const*)X, nb, mean_kin);
+    check_orbitals(ctx, n_blocks, X, "tpa_multi");
+    std::vector<KinDotsItem> v;
+    for (int i = 0; i < n; ++i)
+      v.push_back(KinDotsItem{(const cplx*)X[i], kbs[i]->n_pw, kbs[i]->n_pw, nb, kbs[i]->kin.p, mean_kin + (size_t)i * nb});
+    BatchExec(ctx, ctx->slot[0]).kin_dots_batch(v);
+    finish(ctx);
   }
   if (Q) {                // ldiv!
-    check_dev(n_blocks, Q, "tpa_multi");
-    check_dev(n_blocks, (const void* const*)S, "tpa_multi");
+    check_orbitals(ctx, n_blocks, Q, "tpa_multi");
+    check_orbitals(ctx, n_blocks, (const void* const*)S, "tpa_multi");
     REQUIRE(inv_w_host, "tpa_multi: NULL weights");
     std::vector<DmTpaItem> v;
     long long mt = 1;
@@ -270,9 +286,9 @@ int dftk_b200_tpa_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, const vo
                             use_tpa ? mean_kin + (size_t)i * nb : nullptr, inv_w_host[i]});
       mt = std::max(mt, (long long)kbs[i]->n_pw * nb);
     }
-    LAUNCH(ctx, k_dm_tpa, dim3(grid_for(ctx, mt), (unsigned)n), DM_THREADS, 0, put(ctx, ctx->dm_items, v));
+    LAUNCH(ctx, k_dm_tpa, dim3(grid_for(ctx, mt), (unsigned)n), DM_THREADS, 0, ctx->slot[0].ring.put(v, ctx->stream));
   }
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  finish(ctx);
   API_END(ctx)
 }
 
@@ -286,8 +302,8 @@ int dftk_b200_real_dots_multi(int64_t n_pairs, int64_t n_blocks, dftk_b200_kbloc
     for (int64_t p = 0; p < n_pairs; ++p) out_host[p] = 0.0;
     return DFTK_B200_OK;
   }
-  check_dev(n_pairs * n_blocks, A, "real_dots_multi");
-  check_dev(n_pairs * n_blocks, B, "real_dots_multi");
+  check_orbitals(ctx, n_pairs * n_blocks, A, "real_dots_multi");
+  check_orbitals(ctx, n_pairs * n_blocks, B, "real_dots_multi");
   std::vector<DmDotItem> v;
   for (int64_t p = 0; p < n_pairs; ++p)
     for (int64_t i = 0; i < n_blocks; ++i) {
@@ -305,10 +321,10 @@ int dftk_b200_axpy_dot_multi(int64_t n_blocks, dftk_b200_kblock* const* kbs, voi
   check_blocks(ctx, n_blocks, kbs, n_bands, "axpy_dot_multi");
   if (out_host) *out_host = 0.0;
   if (n_blocks == 0) return DFTK_B200_OK;
-  check_dev(n_blocks, (const void* const*)Y, "axpy_dot_multi");
-  check_dev(n_blocks, X, "axpy_dot_multi");
+  check_orbitals(ctx, n_blocks, (const void* const*)Y, "axpy_dot_multi");
+  check_orbitals(ctx, n_blocks, X, "axpy_dot_multi");
   if (Z) {
-    check_dev(n_blocks, Z, "axpy_dot_multi");
+    check_orbitals(ctx, n_blocks, Z, "axpy_dot_multi");
     REQUIRE(out_host, "axpy_dot_multi: NULL result");
   }
   std::vector<DmDotItem> v;

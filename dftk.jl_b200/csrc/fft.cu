@@ -319,7 +319,7 @@ void kb_apply_local_kinetic(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, i
 }
 
 bool kb_apply_local_kinetic_multi(int n, dftk_b200_kblock* const* kbs, const cplx* const* psi, cplx* const* hpsi,
-                                  const int* n_bands, const void* (*upload)(void* self, const void* host, size_t bytes), void* self) {
+                                  const int* n_bands, DescRing& ring) {
   if (n <= 0) return true;
   dftk_b200_grid* g = kbs[0]->grid;
   dftk_b200_ctx* ctx = g->ctx;
@@ -355,8 +355,9 @@ bool kb_apply_local_kinetic_multi(int n, dftk_b200_kblock* const* kbs, const cpl
     it.kin = kb->kin.p;
     for (int l = 0; l < n_bands[i]; ++l) bandmap[b++] = make_int2(i, l);
   }
-  const FftMultiItem* d_items = (const FftMultiItem*)upload(self, items.data(), items.size() * sizeof(FftMultiItem));
-  const int2* d_map = (const int2*)upload(self, bandmap.data(), bandmap.size() * sizeof(int2));
+  ring.reserve(DescRing::padded(items) + DescRing::padded(bandmap), ctx->stream);
+  const FftMultiItem* d_items = ring.put(items, ctx->stream);
+  const int2* d_map = ring.put(bandmap, ctx->stream);
   {
     int L = reg_L(g->rx), Lp = L + 1;
     const cplx* tw = (const cplx*)g->twx.p;
@@ -396,7 +397,7 @@ bool kb_density_accumulate_multi(int n, dftk_b200_kblock* const* kbs, const cplx
   dftk_b200_grid* g = kbs[0]->grid;
   dftk_b200_ctx* ctx = g->ctx;
   if (!(g->rx && g->ry && g->rz)) return false;
-  int total = 0, max_cols = 0, max_zc = 0, total_w = 0;
+  int total = 0, max_cols = 0, max_zc = 0;
   for (int i = 0; i < n; ++i) {
     dftk_b200_kblock* kb = kbs[i];
     if (kb->grid != g || !kb->T.ranges_ok || kb->spin < 0 || kb->spin > 1) return false;
@@ -408,15 +409,10 @@ bool kb_density_accumulate_multi(int n, dftk_b200_kblock* const* kbs, const cplx
   if (total == 0) return true;
   if (total > 65535) return false;
   // device copies: weights (scaled by ifft_norm^2), items, band map -- staged through the context's descriptor ring
-  std::vector<double> w(total);
+  std::vector<double> w;
   std::vector<FftMultiItem> items;
   std::vector<int2> bandmap;
   const double nrm = g->ifft_norm * g->ifft_norm;
-  size_t need = ((size_t)total * sizeof(double) + 255 & ~(size_t)255) + ((size_t)n * sizeof(FftMultiItem) + 255 & ~(size_t)255) +
-                ((size_t)total * sizeof(int2) + 255 & ~(size_t)255) + 1024;
-  char* ring = ctx->batch_ring.ensure(std::max<size_t>(need, (size_t)4 << 20));
-  double* d_w = (double*)ring;
-  size_t off_items = ((size_t)total * sizeof(double) + 255) & ~(size_t)255;
   for (int i = 0; i < n; ++i) {
     dftk_b200_kblock* kb = kbs[i];
     if (n_bands[i] <= 0) continue;
@@ -427,26 +423,25 @@ bool kb_density_accumulate_multi(int n, dftk_b200_kblock* const* kbs, const cplx
     it.ldpsi = kb->n_pw;
     it.W1 = kb->W1.p;
     it.W2 = kb->W2.p;
-    it.wts = d_w + total_w;
     it.nb = n_bands[i];
     it.V = nullptr;
     it.out = nullptr;
     it.kin = (const double*)(intptr_t)kb->spin;      // spin channel of the block rides in an unused pointer slot
     for (int l = 0; l < n_bands[i]; ++l) {
-      w[total_w + l] = occ_w_host[(size_t)i * ld_w + l] * nrm;
+      w.push_back(occ_w_host[(size_t)i * ld_w + l] * nrm);
       bandmap.push_back(make_int2((int)items.size(), l));
     }
-    total_w += n_bands[i];
     items.push_back(it);
   }
-  FftMultiItem* d_items = (FftMultiItem*)(ring + off_items);
-  size_t off_map = off_items + (((size_t)items.size() * sizeof(FftMultiItem) + 255) & ~(size_t)255);
-  int2* d_map = (int2*)(ring + off_map);
-  CUDA_CHECK(cudaMemcpyAsync(d_w, w.data(), (size_t)total * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_CHECK(cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(FftMultiItem), cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_CHECK(cudaMemcpyAsync(d_map, bandmap.data(), bandmap.size() * sizeof(int2), cudaMemcpyHostToDevice, ctx->stream));
-  const FftMultiItem* c_items = d_items;
-  const int2* c_map = d_map;
+  DescRing& ring = ctx->slot[0].ring;
+  ring.reserve(DescRing::padded(w) + DescRing::padded(items) + DescRing::padded(bandmap), ctx->stream);
+  const double* d_w = ring.put(w, ctx->stream);
+  for (auto& it : items) {
+    it.wts = d_w;
+    d_w += it.nb;
+  }
+  const FftMultiItem* c_items = ring.put(items, ctx->stream);
+  const int2* c_map = ring.put(bandmap, ctx->stream);
   {
     int L = reg_L(g->rx), Lp = L + 1;
     const cplx* tw = (const cplx*)g->twx.p;
@@ -471,7 +466,8 @@ bool kb_density_accumulate_multi(int n, dftk_b200_kblock* const* kbs, const cplx
     void* args[] = {&c_items, &n_items, &spin, &tw, &r, &L, &Lp};
     launch_ptr(ctx, g->rz->m_z_density, dim3(cdiv(g->nx, L), g->ny), L * g->rz->T, sm, args);
   }
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));     // host staging vectors go out of scope
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ring.rewind();
   return true;
 }
 
@@ -528,7 +524,8 @@ void kb_density_accumulate(dftk_b200_kblock* kb, const cplx* psi, const double* 
   if (n_bands == 0) return;
   std::vector<double> w(n_bands);
   for (int64_t i = 0; i < n_bands; ++i) w[i] = occ_w_host[i] * g->ifft_norm * g->ifft_norm;
-  kb->wts.upload(w.data(), n_bands, ctx->stream);
+  DescRing& ring = ctx->slot[0].ring;
+  const double* w_dev = ring.put(w, ctx->stream);
   const int chunk = band_chunk_for(kb, n_bands);
   for (int64_t b0 = 0; b0 < n_bands; b0 += chunk) {
     int nb = (int)std::min<int64_t>(chunk, n_bands - b0);
@@ -537,7 +534,7 @@ void kb_density_accumulate(dftk_b200_kblock* kb, const cplx* psi, const double* 
       int L = reg_L(g->rz), Lp = L + 1;
       const cplx* tw = (const cplx*)g->twz.p;
       const cplx* W2 = kb->W2.p;
-      const double* wp = kb->wts.p + b0;
+      const double* wp = w_dev + b0;
       size_t sm = reg_smem(g->rz) + (size_t)g->nz * L * sizeof(double);
       void* args[] = {&kb->T, &tw, &W2, &wp, &nb, &rho, &L, &Lp};
       launch_ptr(ctx, g->rz->z_density, dim3(cdiv(g->nx, L), g->ny), L * g->rz->T, sm, args);
@@ -545,11 +542,11 @@ void kb_density_accumulate(dftk_b200_kblock* kb, const cplx* psi, const double* 
       int L = g->Lz, Lp = L | 1;
       size_t sm = smem_for(g->nz, L) + (size_t)g->nz * L * sizeof(double);
       LAUNCH(ctx, k_z_density, dim3(cdiv(g->nx, L), g->ny), FFT_THREADS, sm, kb->T, g->pz,
-             (const cplx*)g->twz.p, (const cplx*)kb->W2.p, (const double*)(kb->wts.p + b0), nb, rho, L, Lp);
+             (const cplx*)g->twz.p, (const cplx*)kb->W2.p, w_dev + b0, nb, rho, L, Lp);
     }
   }
-  // the host weight vector must outlive the async upload
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ring.rewind();
 }
 
 }  // namespace dftk

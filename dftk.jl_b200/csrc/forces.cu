@@ -262,7 +262,8 @@ void kb_nonlocal_force_rows(dftk_b200_kblock* kb, const cplx* psi, const double*
   cplx* proj = kb->proj.ensure((size_t)5 * np * chunk);     // P'psi | D P'psi | P'(p_α psi) α = 0..2
   cplx* dproj = proj + (size_t)np * chunk;
   cplx* pa = proj + (size_t)2 * np * chunk;
-  kb->wts.upload(occ_w_host, n_bands, ctx->stream);
+  DescRing& ring = ctx->slot[0].ring;
+  const double* w_dev = (const double*)ring.put(occ_w_host, (size_t)n_bands * sizeof(double), ctx->stream);
   double* f = ctx->scal.ensure((size_t)3 * np + 8);
   CUDA_CHECK(cudaMemsetAsync(f, 0, (size_t)3 * np * sizeof(double), ctx->stream));
   const cplx one = make_double2(1.0, 0.0), zero = make_double2(0.0, 0.0);
@@ -275,10 +276,11 @@ void kb_nonlocal_force_rows(dftk_b200_kblock* kb, const cplx* psi, const double*
     zgemm(ctx, 0, np, nb, np, one, kb->Dc.p, np, proj, np, zero, dproj, np);
     zgemm(ctx, 2, np, 3 * nb, n_pw, one, kb->P.p, n_pw, scaled, n_pw, zero, pa, np);
     LAUNCH(ctx, k_nonlocal_force_rows, dim3((unsigned)((np + 127) / 128), 3), 128, 0, np, nb, (const cplx*)dproj,
-           (const cplx*)pa, (const double*)(kb->wts.p + b0), f);
+           (const cplx*)pa, w_dev + b0, f);
   }
   CUDA_CHECK(cudaMemcpyAsync(out_host, f, (size_t)3 * np * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ring.rewind();
 }
 
 }  // namespace dftk

@@ -27,15 +27,6 @@ __global__ void k_ldos_abs2(const cplx* __restrict__ cube, long long total, doub
   }
 }
 
-void check_device_array(dftk_b200_ctx* ctx, const void* p, const char* what) {
-  cudaPointerAttributes a;
-  const cudaError_t e = cudaPointerGetAttributes(&a, p);
-  if (e != cudaSuccess) cudaGetLastError();
-  REQUIRE(p && e == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged),
-          std::string("ldos_accumulate_multi: ") + what + " must be device memory");
-  REQUIRE(a.device == ctx->device, std::string("ldos_accumulate_multi: ") + what + " must be on the context's device");
-}
-
 struct Piece {      // bands [b0, b0 + nb) of block i, all kept
   int i;
   int b0, nb;
@@ -57,10 +48,10 @@ int dftk_b200_ldos_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const* k
   for (int64_t i = 0; i < n_blocks; ++i) {
     REQUIRE(kbs[i] && kbs[i]->grid == g && kbs[i]->spin >= 0 && kbs[i]->spin < n_spin && n_bands[i] >= 0 && n_bands[i] <= ld_w,
             "ldos_accumulate_multi: the blocks must share one grid, with spins below n_spin and n_bands <= ld_w");
-    if (n_bands[i] > 0) check_device_array(ctx, psi[i], "orbitals");
+    if (n_bands[i] > 0) require_device(ctx, psi[i], "ldos_accumulate_multi: orbitals");
   }
-  check_device_array(ctx, W, "W");
-  check_device_array(ctx, ldos, "ldos");
+  require_device(ctx, W, "ldos_accumulate_multi: W");
+  require_device(ctx, ldos, "ldos_accumulate_multi: ldos");
   // screening: a band with a zero weight at every energy is neither transformed nor multiplied
   const int64_t ldw_e = n_blocks * ld_w;           // W[j * ldw_e + i * ld_w + n]
   std::vector<double> Wh((size_t)n_energies * ldw_e);
@@ -120,8 +111,7 @@ int dftk_b200_ldos_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const* k
     }
     o += 2 * K;
   }
-  const double** d_ptrs = (const double**)ctx->ldos_items.ensure(ptrs.size() * sizeof(const double*));
-  CUDA_CHECK(cudaMemcpyAsync(d_ptrs, ptrs.data(), ptrs.size() * sizeof(const double*), cudaMemcpyHostToDevice, ctx->stream));
+  const double* const* d_ptrs = ctx->slot[0].ring.put(ptrs, ctx->stream);
   const double nrm = g->ifft_norm * g->ifft_norm;
   const size_t smem = LD_SMEM_DOUBLES * sizeof(double);      // 53 KB: above the default limit of 48 KB
   CUDA_CHECK(cudaFuncSetAttribute(k_ldos_product, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -148,7 +138,8 @@ int dftk_b200_ldos_accumulate_multi(int64_t n_blocks, dftk_b200_kblock* const* k
     LAUNCH(ctx, k_ldos_product, dim3((unsigned)((g->N + LD_TM - 1) / LD_TM), (unsigned)((n_energies + LD_TN - 1) / LD_TN)),
            LD_THREADS, smem, p);
   }
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));     // the pointer lists are host vectors
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ctx->slot[0].ring.rewind();
   API_END(ctx)
 }
 

@@ -147,7 +147,6 @@ enum OpType {
   OP_GRAM = 0, OP_CHOL, OP_RMUL, OP_BTIMES, OP_HEEV, OP_RESIDUAL, OP_PRECOND, OP_COLNORMS, OP_SCALE, OP_COPY2D, OP_MAKECP,
   OP_STATS, OP_RANDN, OP_LAMBDA, OP_APPLYH, OP_D2H, OP_NTYPES
 };
-struct ApplyHItem { dftk_b200_kblock* kb; const cplx* in; cplx* out; int ncols; };
 struct D2HItem { const double* src; int n; double* host_dst; };
 struct Op {
   int type;
@@ -204,9 +203,8 @@ static void small_gram_geometry(dftk_b200_ctx* ctx, int64_t rows, int* n_ctas_ou
   *n_ctas_out = (int)n_ctas;
   *rpc_out = rpc;
 }
-// One Gram item C = A' B of single tall blocks, with the CTA geometry of the batched kernel.
-static GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB,
-                                 int64_t n_rows, cplx* C) {
+GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB,
+                          int64_t n_rows, cplx* C) {
   GramItem g{};
   g.A.n = g.B.n = 1;
   g.A.p[0] = A; g.A.ld[0] = lda; g.A.cols[0] = nA;
@@ -219,10 +217,8 @@ static GramItem single_gram_item(dftk_b200_ctx* ctx, const cplx* A, int64_t lda,
   g.ldc = nA;
   return g;
 }
-// One update item out = alpha Y c + beta out of a single tall block Y (n_rows x nY, like out of leading dimension n_rows;
-// c is nY x ncols, packed).
-static BtimesItem single_btimes_item(const cplx* Y, int nY, const cplx* c, int ncols, cplx* out, int64_t n_rows, double alpha,
-                                     double beta) {
+BtimesItem single_btimes_item(const cplx* Y, int nY, const cplx* c, int ncols, cplx* out, int64_t n_rows, double alpha,
+                              double beta) {
   BtimesItem b{};
   b.Y.n = 1;
   b.Y.p[0] = Y; b.Y.ld[0] = n_rows; b.Y.cols[0] = nY;
@@ -232,325 +228,241 @@ static BtimesItem single_btimes_item(const cplx* Y, int nY, const cplx* c, int n
   return b;
 }
 
-// Launches the recorded operations: the same operation of several solves becomes one launch.
-struct BatchExec {
-  dftk_b200_ctx* ctx;
-  char* ring_h = nullptr;      // pinned staging of the item descriptors
-  size_t ring_cap = 0, ring_off = 0;
-  double* gather_h = nullptr;  // pinned landing zone of the per-round D2H gather
-  size_t gather_cap = 0;
-  std::vector<std::pair<double*, std::pair<size_t, int>>> scatter;   // host_dst <- gather_h[offset .. offset+n)
-  size_t gather_used = 0;
-  int64_t rounds = 0;
+BatchExec::BatchExec(dftk_b200_ctx* c, BatchSlot& s) : ctx(c), slot(s) {
+  // pinned staging is created once per slot (cudaMallocHost costs about a millisecond)
+  if (!slot.gather_h) CUDA_CHECK(cudaMallocHost((void**)&slot.gather_h, BatchSlot::GATHER_CAP * sizeof(double)));
+  slot.gather.ensure(BatchSlot::GATHER_CAP);
+  if (!slot.ev) CUDA_CHECK(cudaEventCreateWithFlags(&slot.ev, cudaEventDisableTiming));
+}
+void BatchExec::reset_counters(size_t n) {
+  slot.counter.ensure(std::max<size_t>(n, 256));
+  CUDA_CHECK(cudaMemsetAsync(slot.counter.p, 0, slot.counter.cap * sizeof(int), ctx->stream));
+}
 
-  // the executor's device-side buffers: group 0 = the context's, group 1 = the second set (pipelined batches)
-  DevBuf<char>* ring_d = nullptr;
-  DevBuf<double>* gather_d = nullptr;
-  DevBuf<char>* ws_d = nullptr;
-  DevBuf<int>* counter_d = nullptr;
-  cudaEvent_t ev = nullptr;
-  bool in_flight = false;
+void BatchExec::gram_batch(std::vector<GramItem>& v) {
+  // per-item partial workspaces and arrival counters
+  size_t ws_total = 0;
+  int max_ctas = 1;
+  size_t smem = 0;
+  for (auto& it : v) {
+    const int nA = it.A.start[it.A.n], nB = it.B.start[it.B.n];
+    ws_total += (size_t)it.n_ctas * nA * nB;
+    max_ctas = std::max(max_ctas, it.n_ctas);
+    smem = std::max(smem, (size_t)SMALL_TR * (nA + nB) * sizeof(cplx));
+  }
+  cplx* ws = (cplx*)slot.gram_ws->ensure(ws_total * sizeof(cplx));
+  if (slot.counter.cap < v.size()) reset_counters(v.size());
+  size_t off = 0;
+  for (size_t i = 0; i < v.size(); ++i) {
+    const int nA = v[i].A.start[v[i].A.n], nB = v[i].B.start[v[i].B.n];
+    v[i].ws = ws + off;
+    v[i].counter = (unsigned*)slot.counter.p + i;
+    off += (size_t)v[i].n_ctas * nA * nB;
+  }
+  const GramItem* d = upload(v);
+  LAUNCH(ctx, kb_gram, dim3((unsigned)max_ctas, (unsigned)v.size()), 256, smem, d);
+}
+void BatchExec::btimes_batch(const std::vector<BtimesItem>& v) {
+  long long max_rows = 1;
+  size_t smem = 0;
+  for (auto& it : v) {
+    max_rows = std::max(max_rows, it.n_rows);
+    smem = std::max(smem, (size_t)it.Y.start[it.Y.n] * it.ncols * sizeof(cplx));
+  }
+  const BtimesItem* d = upload(v);
+  LAUNCH(ctx, kb_btimes, dim3((unsigned)((max_rows + 127) / 128), (unsigned)v.size()), 128, smem, d);
+}
+void BatchExec::heev_batch(const std::vector<HeevItem>& v) {
+  size_t smem = 0;
+  for (auto& it : v) {
+    const size_t half = ((it.n + 1) & ~1) / 2;
+    smem = std::max(smem, (size_t)it.n * it.n * sizeof(cplx) + 2 * (half + 1) * sizeof(cplx) + SMALL_RED * sizeof(double) +
+                              2 * (half + 1) * sizeof(int) + 16);
+  }
+  LAUNCH(ctx, kb_heev, (unsigned)v.size(), SMALL_RED, smem, upload(v));
+}
+void BatchExec::kin_dots_batch(const std::vector<KinDotsItem>& v) {
+  int mc = 1;
+  for (auto& it : v) mc = std::max(mc, it.n_cols);
+  LAUNCH(ctx, kb_kin_dots, dim3((unsigned)mc, (unsigned)v.size()), 256, 0, upload(v));
+}
+// local + kinetic part: the k-block's own batched FFT pipeline; nonlocal part P (D P'psi) as two batched small products
+// over all items (projector counts of the small configurations are <= 20)
+void BatchExec::apply_h_batch(const std::vector<ApplyHItem>& v) {
+  {
+    // local + kinetic part of all k-blocks in five launches when they share the grid's register FFT engine
+    std::vector<dftk_b200_kblock*> kbs;
+    std::vector<const cplx*> in;
+    std::vector<cplx*> out;
+    std::vector<int> nb;
+    for (const ApplyHItem& a : v) {
+      kbs.push_back(a.kb); in.push_back(a.in); out.push_back(a.out); nb.push_back(a.ncols);
+    }
+    if (!kb_apply_local_kinetic_multi((int)kbs.size(), kbs.data(), in.data(), out.data(), nb.data(), slot.ring))
+      for (const ApplyHItem& a : v) kb_apply_local_kinetic(a.kb, a.in, a.out, a.ncols, a.kb->has_V, a.kb->has_kin, false);
+  }
+  std::vector<GramItem> g;
+  std::vector<BtimesItem> b;
+  for (const ApplyHItem& a : v) {
+    dftk_b200_kblock* kb = a.kb;
+    if (kb->n_nl() == 0) continue;
+    if (kb->n_nl() > SMALL_MAX_COLS || a.ncols > SMALL_MAX_N || !kb->PD.p) {
+      kb_apply_nonlocal(kb, a.in, a.out, a.ncols);
+      continue;
+    }
+    cplx* proj = kb->proj.ensure((size_t)2 * kb->n_nl() * SMALL_MAX_N);
+    const int nl = (int)kb->n_nl();
+    g.push_back(single_gram_item(ctx, kb->P.p, kb->n_pw, nl, a.in, kb->n_pw, a.ncols, kb->n_pw, proj));
+    b.push_back(single_btimes_item(kb->PD.p, nl, proj, a.ncols, a.out, kb->n_pw, 1.0, 1.0));
+  }
+  if (!g.empty()) {
+    gram_batch(g);
+    btimes_batch(b);
+  }
+}
 
-  explicit BatchExec(dftk_b200_ctx* c, int group = 0) : ctx(c) {
-    // pinned staging buffers are created once per context (cudaMallocHost costs about a millisecond)
-    ring_cap = (size_t)4 << 20;
-    gather_cap = (size_t)1 << 18;
-    char** rh = group ? &ctx->batch_ring_h2 : &ctx->batch_ring_h;
-    double** gh = group ? &ctx->batch_gather_h2 : &ctx->batch_gather_h;
-    if (!*rh) {
-      CUDA_CHECK(cudaMallocHost((void**)rh, ring_cap));
-      CUDA_CHECK(cudaMallocHost((void**)gh, gather_cap * sizeof(double)));
+void BatchExec::launch(int type, const std::vector<Op*>& ops) {
+  const unsigned n = (unsigned)ops.size();
+  switch (type) {
+    case OP_GRAM: {
+      auto v = collect<GramItem>(ops, [](Op* o) { return o->u.gram; });
+      gram_batch(v);
+      break;
     }
-    ring_h = *rh;
-    gather_h = *gh;
-    ring_d = group ? &ctx->batch_ring2 : &ctx->batch_ring;
-    gather_d = group ? &ctx->batch_gather2 : &ctx->batch_gather;
-    ws_d = group ? &ctx->batch_ws2 : &ctx->gemm_ws;
-    counter_d = group ? &ctx->small_counter2 : &ctx->small_counter;
-    ring_d->ensure(ring_cap);
-    gather_d->ensure(gather_cap);
-    if (!ctx->batch_events[group]) CUDA_CHECK(cudaEventCreateWithFlags(&ctx->batch_events[group], cudaEventDisableTiming));
-    ev = ctx->batch_events[group];
-  }
-  // arrival counters of kb_gram, zeroed (also recovers from an aborted solve)
-  void reset_counters(size_t n) {
-    counter_d->ensure(std::max<size_t>(n, 256));
-    CUDA_CHECK(cudaMemsetAsync(counter_d->p, 0, counter_d->cap * sizeof(int), ctx->stream));
-  }
-  BatchExec(const BatchExec&) = delete;
-  BatchExec& operator=(const BatchExec&) = delete;
-
-  // copy `n` descriptors to the device ring; returns the device address.  The ring is recycled at every stream
-  // synchronisation (the staging memory of an enqueued copy must stay untouched until the copy has run).
-  const void* upload_bytes(const void* host, size_t n_bytes) {
-    const size_t bytes = (n_bytes + 255) & ~(size_t)255;
-    if (ring_off + bytes > ring_cap) {
-      CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-      ring_off = 0;
-      REQUIRE(bytes <= ring_cap, "batched LOBPCG: descriptor ring too small");
+    case OP_CHOL: {
+      auto v = collect<CholItem>(ops, [](Op* o) { return o->u.chol; });
+      LAUNCH(ctx, kb_chol, n, SMALL_RED, 0, upload(v));
+      break;
     }
-    memcpy(ring_h + ring_off, host, n_bytes);
-    char* d = ring_d->p + ring_off;
-    CUDA_CHECK(cudaMemcpyAsync(d, ring_h + ring_off, n_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ring_off += bytes;
-    return d;
-  }
-  template <class T>
-  const T* upload(const std::vector<T>& items) {
-    return (const T*)upload_bytes(items.data(), items.size() * sizeof(T));
-  }
-  template <class T, class F>
-  std::vector<T> collect(const std::vector<Op*>& ops, F get) {
-    std::vector<T> v;
-    v.reserve(ops.size());
-    for (Op* o : ops) v.push_back(get(o));
-    return v;
-  }
-  unsigned gx_for(long long total) const {
-    long long g = (total + 255) / 256;
-    return (unsigned)std::max<long long>(1, std::min<long long>(g, (long long)ctx->sm_count * 32));
-  }
-
-  void gram_batch(std::vector<GramItem>& v) {
-    // per-item partial workspaces and arrival counters
-    size_t ws_total = 0;
-    int max_ctas = 1;
-    size_t smem = 0;
-    for (auto& it : v) {
-      const int nA = it.A.start[it.A.n], nB = it.B.start[it.B.n];
-      ws_total += (size_t)it.n_ctas * nA * nB;
-      max_ctas = std::max(max_ctas, it.n_ctas);
-      smem = std::max(smem, (size_t)SMALL_TR * (nA + nB) * sizeof(cplx));
+    case OP_RMUL: {
+      auto v = collect<RmulItem>(ops, [](Op* o) { return o->u.rmul; });
+      long long max_rows = 1;
+      size_t smem = 0;
+      for (auto& it : v) {
+        max_rows = std::max(max_rows, it.n_rows);
+        smem = std::max(smem, (size_t)it.n * it.n * sizeof(cplx));
+      }
+      LAUNCH(ctx, kb_rmul, dim3((unsigned)((max_rows + 127) / 128), n), 128, smem, upload(v));
+      break;
     }
-    cplx* ws = (cplx*)ws_d->ensure(ws_total * sizeof(cplx));
-    if (counter_d->cap < v.size()) reset_counters(v.size());
-    size_t off = 0;
-    for (size_t i = 0; i < v.size(); ++i) {
-      const int nA = v[i].A.start[v[i].A.n], nB = v[i].B.start[v[i].B.n];
-      v[i].ws = ws + off;
-      v[i].counter = (unsigned*)counter_d->p + i;
-      off += (size_t)v[i].n_ctas * nA * nB;
+    case OP_BTIMES: btimes_batch(collect<BtimesItem>(ops, [](Op* o) { return o->u.btimes; })); break;
+    case OP_HEEV: heev_batch(collect<HeevItem>(ops, [](Op* o) { return o->u.heev; })); break;
+    case OP_RESIDUAL: {
+      auto v = collect<ResidualItem>(ops, [](Op* o) { return o->u.residual; });
+      int mc = 1;
+      for (auto& it : v) mc = std::max(mc, it.n_cols);
+      LAUNCH(ctx, kb_residual, dim3((unsigned)mc, n), 256, 0, upload(v));
+      break;
     }
-    const GramItem* d = upload(v);
-    LAUNCH(ctx, kb_gram, dim3((unsigned)max_ctas, (unsigned)v.size()), 256, smem, d);
-  }
-  void btimes_batch(const std::vector<BtimesItem>& v) {
-    long long max_rows = 1;
-    size_t smem = 0;
-    for (auto& it : v) {
-      max_rows = std::max(max_rows, it.n_rows);
-      smem = std::max(smem, (size_t)it.Y.start[it.Y.n] * it.ncols * sizeof(cplx));
+    case OP_LAMBDA: {
+      auto v = collect<LambdaItem>(ops, [](Op* o) { return o->u.lambda; });
+      int mc = 1;
+      for (auto& it : v) mc = std::max(mc, it.n_cols);
+      LAUNCH(ctx, kb_lambda, dim3((unsigned)mc, n), 256, 0, upload(v));
+      break;
     }
-    const BtimesItem* d = upload(v);
-    LAUNCH(ctx, kb_btimes, dim3((unsigned)((max_rows + 127) / 128), (unsigned)v.size()), 128, smem, d);
-  }
-
-  void launch(int type, const std::vector<Op*>& ops) {
-    const unsigned n = (unsigned)ops.size();
-    switch (type) {
-      case OP_GRAM: {
-        auto v = collect<GramItem>(ops, [](Op* o) { return o->u.gram; });
-        gram_batch(v);
-        break;
-      }
-      case OP_CHOL: {
-        auto v = collect<CholItem>(ops, [](Op* o) { return o->u.chol; });
-        LAUNCH(ctx, kb_chol, n, SMALL_RED, 0, upload(v));
-        break;
-      }
-      case OP_RMUL: {
-        auto v = collect<RmulItem>(ops, [](Op* o) { return o->u.rmul; });
-        long long max_rows = 1;
-        size_t smem = 0;
-        for (auto& it : v) {
-          max_rows = std::max(max_rows, it.n_rows);
-          smem = std::max(smem, (size_t)it.n * it.n * sizeof(cplx));
-        }
-        LAUNCH(ctx, kb_rmul, dim3((unsigned)((max_rows + 127) / 128), n), 128, smem, upload(v));
-        break;
-      }
-      case OP_BTIMES: {
-        auto v = collect<BtimesItem>(ops, [](Op* o) { return o->u.btimes; });
-        btimes_batch(v);
-        break;
-      }
-      case OP_HEEV: {
-        auto v = collect<HeevItem>(ops, [](Op* o) { return o->u.heev; });
-        size_t smem = 0;
-        for (auto& it : v) {
-          const size_t half = ((it.n + 1) & ~1) / 2;
-          smem = std::max(smem, (size_t)it.n * it.n * sizeof(cplx) + 2 * (half + 1) * sizeof(cplx) + SMALL_RED * sizeof(double) +
-                                    2 * (half + 1) * sizeof(int) + 16);
-        }
-        LAUNCH(ctx, kb_heev, n, SMALL_RED, smem, upload(v));
-        break;
-      }
-      case OP_RESIDUAL: {
-        auto v = collect<ResidualItem>(ops, [](Op* o) { return o->u.residual; });
-        int mc = 1;
-        for (auto& it : v) mc = std::max(mc, it.n_cols);
-        LAUNCH(ctx, kb_residual, dim3((unsigned)mc, n), 256, 0, upload(v));
-        break;
-      }
-      case OP_LAMBDA: {
-        auto v = collect<LambdaItem>(ops, [](Op* o) { return o->u.lambda; });
-        int mc = 1;
-        for (auto& it : v) mc = std::max(mc, it.n_cols);
-        LAUNCH(ctx, kb_lambda, dim3((unsigned)mc, n), 256, 0, upload(v));
-        break;
-      }
-      case OP_COLNORMS: {
-        auto v = collect<ColnormItem>(ops, [](Op* o) { return o->u.colnorm; });
-        int mc = 1;
-        for (auto& it : v) mc = std::max(mc, it.n_cols);
-        LAUNCH(ctx, kb_col_norms, dim3((unsigned)mc, n), 256, 0, upload(v));
-        break;
-      }
-      case OP_PRECOND: {
-        auto v = collect<PrecondItem>(ops, [](Op* o) { return o->u.precond; });
-        long long mt = 1;
-        for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
-        LAUNCH(ctx, kb_precondition, dim3(gx_for(mt), n), 256, 0, upload(v));
-        break;
-      }
-      case OP_SCALE: {
-        auto v = collect<ScaleItem>(ops, [](Op* o) { return o->u.scale; });
-        long long mt = 1;
-        for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
-        LAUNCH(ctx, kb_scale_cols_inv, dim3(gx_for(mt), n), 256, 0, upload(v));
-        break;
-      }
-      case OP_COPY2D: {
-        auto v = collect<Copy2dItem>(ops, [](Op* o) { return o->u.copy2d; });
-        long long mt = 1;
-        for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
-        LAUNCH(ctx, kb_copy2d, dim3(gx_for(mt), n), 256, 0, upload(v));
-        break;
-      }
-      case OP_MAKECP: {
-        auto v = collect<MakecpItem>(ops, [](Op* o) { return o->u.makecp; });
-        long long mt = 1;
-        for (auto& it : v) mt = std::max(mt, (long long)it.n_rows * it.n_cols);
-        LAUNCH(ctx, kb_make_cP, dim3(gx_for(mt), n), 256, 0, upload(v));
-        break;
-      }
-      case OP_STATS: {
-        auto v = collect<StatsItem>(ops, [](Op* o) { return o->u.stats; });
-        LAUNCH(ctx, kb_matrix_stats, n, 256, 0, upload(v));
-        break;
-      }
-      case OP_RANDN: {
-        auto v = collect<RandnItem>(ops, [](Op* o) { return o->u.randn; });
-        long long mt = 1;
-        for (auto& it : v) mt = std::max(mt, it.n_rows);
-        LAUNCH(ctx, kb_randn_col, dim3(gx_for(mt), n), 256, 0, upload(v));
-        break;
-      }
-      case OP_APPLYH: {
-        // local + kinetic part: the k-block's own batched FFT pipeline; nonlocal part P (D P'psi) as two batched small
-        // products over all k-blocks of the round (projector counts of the small configurations are <= 20)
-        std::vector<GramItem> g;
-        std::vector<BtimesItem> b;
-        {
-          // local + kinetic part of all k-blocks in five launches when they share the grid's register FFT engine
-          std::vector<dftk_b200_kblock*> kbs;
-          std::vector<const cplx*> in;
-          std::vector<cplx*> out;
-          std::vector<int> nb;
-          for (Op* o : ops) {
-            const ApplyHItem& a = o->u.applyh;
-            kbs.push_back(a.kb); in.push_back(a.in); out.push_back(a.out); nb.push_back(a.ncols);
-          }
-          auto up = [](void* self, const void* host, size_t bytes) -> const void* {
-            return ((BatchExec*)self)->upload_bytes(host, bytes);
-          };
-          if (!kb_apply_local_kinetic_multi((int)kbs.size(), kbs.data(), in.data(), out.data(), nb.data(), up, this))
-            for (Op* o : ops) {
-              const ApplyHItem& a = o->u.applyh;
-              kb_apply_local_kinetic(a.kb, a.in, a.out, a.ncols, a.kb->has_V, a.kb->has_kin, false);
-            }
-        }
-        for (Op* o : ops) {
-          const ApplyHItem& a = o->u.applyh;
-          dftk_b200_kblock* kb = a.kb;
-          if (kb->n_nl() == 0) continue;
-          if (kb->n_nl() > SMALL_MAX_COLS || a.ncols > SMALL_MAX_N || !kb->PD.p) {
-            kb_apply_nonlocal(kb, a.in, a.out, a.ncols);
-            continue;
-          }
-          cplx* proj = kb->proj.ensure((size_t)2 * kb->n_nl() * SMALL_MAX_N);
-          const int nl = (int)kb->n_nl();
-          g.push_back(single_gram_item(ctx, kb->P.p, kb->n_pw, nl, a.in, kb->n_pw, a.ncols, kb->n_pw, proj));
-          b.push_back(single_btimes_item(kb->PD.p, nl, proj, a.ncols, a.out, kb->n_pw, 1.0, 1.0));
-        }
-        if (!g.empty()) {
-          gram_batch(g);
-          btimes_batch(b);
-        }
-        break;
-      }
-      case OP_D2H: {
-        std::vector<GatherItem> v;
-        for (Op* o : ops) {
-          const D2HItem& d = o->u.d2h;
-          REQUIRE(gather_used + d.n <= gather_cap, "batched LOBPCG: gather buffer too small");
-          v.push_back(GatherItem{d.src, d.n, (int)gather_used});
-          scatter.push_back({d.host_dst, {gather_used, d.n}});
-          gather_used += d.n;
-        }
-        LAUNCH(ctx, kb_gather, n, 64, 0, upload(v), gather_d->p);
-        break;
-      }
-      default: throw Error(DFTK_B200_EINVAL, "batched LOBPCG: unknown operation");
+    case OP_COLNORMS: {
+      auto v = collect<ColnormItem>(ops, [](Op* o) { return o->u.colnorm; });
+      int mc = 1;
+      for (auto& it : v) mc = std::max(mc, it.n_cols);
+      LAUNCH(ctx, kb_col_norms, dim3((unsigned)mc, n), 256, 0, upload(v));
+      break;
     }
-  }
-  // run everything recorded by the solves since the last round; one stream synchronisation at the end
-  void flush(std::vector<Coro*>& coros) {
-    issue(coros);
-    complete(coros);
-  }
-  // enqueue everything recorded by the solves since the last round (launches + the round's result gather) on ctx->stream
-  void issue(std::vector<Coro*>& coros) {
-    bool any = false;
-    for (auto& c : coros) any = any || c->cursor < c->ops.size();
-    if (!any) return;
-    rounds++;
-    std::vector<Op*> batch;
-    while (true) {
-      // count the operation types at the cursors; run the rarest one first so that solves that are an operation behind
-      // (a retry, a re-randomised column) catch up with the pack
-      int count[OP_NTYPES] = {0};
-      for (auto& c : coros)
-        if (c->cursor < c->ops.size()) count[c->ops[c->cursor].type]++;
-      int best = -1;
-      for (int t = 0; t < OP_NTYPES; ++t)
-        if (count[t] > 0 && (best < 0 || count[t] < count[best])) best = t;
-      if (best < 0) break;
-      batch.clear();
-      for (auto& c : coros)
-        if (c->cursor < c->ops.size() && c->ops[c->cursor].type == best) batch.push_back(&c->ops[c->cursor++]);
-      launch(best, batch);
+    case OP_PRECOND: {
+      auto v = collect<PrecondItem>(ops, [](Op* o) { return o->u.precond; });
+      long long mt = 1;
+      for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
+      LAUNCH(ctx, kb_precondition, dim3(gx_for(mt), n), 256, 0, upload(v));
+      break;
     }
-    if (gather_used)
-      CUDA_CHECK(cudaMemcpyAsync(gather_h, gather_d->p, gather_used * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDA_CHECK(cudaEventRecord(ev, ctx->stream));
-    in_flight = true;
-  }
-  // wait for the issued round, hand the gathered values to the solves
-  void complete(std::vector<Coro*>& coros) {
-    if (!in_flight) return;
-    CUDA_CHECK(cudaEventSynchronize(ev));
-    in_flight = false;
-    for (auto& s : scatter) memcpy(s.first, gather_h + s.second.first, s.second.second * sizeof(double));
-    scatter.clear();
-    gather_used = 0;
-    ring_off = 0;
-    for (auto& c : coros) {
-      c->ops.clear();
-      c->cursor = 0;
+    case OP_SCALE: {
+      auto v = collect<ScaleItem>(ops, [](Op* o) { return o->u.scale; });
+      long long mt = 1;
+      for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
+      LAUNCH(ctx, kb_scale_cols_inv, dim3(gx_for(mt), n), 256, 0, upload(v));
+      break;
     }
+    case OP_COPY2D: {
+      auto v = collect<Copy2dItem>(ops, [](Op* o) { return o->u.copy2d; });
+      long long mt = 1;
+      for (auto& it : v) mt = std::max(mt, it.n_rows * it.n_cols);
+      LAUNCH(ctx, kb_copy2d, dim3(gx_for(mt), n), 256, 0, upload(v));
+      break;
+    }
+    case OP_MAKECP: {
+      auto v = collect<MakecpItem>(ops, [](Op* o) { return o->u.makecp; });
+      long long mt = 1;
+      for (auto& it : v) mt = std::max(mt, (long long)it.n_rows * it.n_cols);
+      LAUNCH(ctx, kb_make_cP, dim3(gx_for(mt), n), 256, 0, upload(v));
+      break;
+    }
+    case OP_STATS: {
+      auto v = collect<StatsItem>(ops, [](Op* o) { return o->u.stats; });
+      LAUNCH(ctx, kb_matrix_stats, n, 256, 0, upload(v));
+      break;
+    }
+    case OP_RANDN: {
+      auto v = collect<RandnItem>(ops, [](Op* o) { return o->u.randn; });
+      long long mt = 1;
+      for (auto& it : v) mt = std::max(mt, it.n_rows);
+      LAUNCH(ctx, kb_randn_col, dim3(gx_for(mt), n), 256, 0, upload(v));
+      break;
+    }
+    case OP_APPLYH: apply_h_batch(collect<ApplyHItem>(ops, [](Op* o) { return o->u.applyh; })); break;
+    case OP_D2H: {
+      std::vector<GatherItem> v;
+      for (Op* o : ops) {
+        const D2HItem& d = o->u.d2h;
+        REQUIRE(gather_used + d.n <= BatchSlot::GATHER_CAP, "batched LOBPCG: gather buffer too small");
+        v.push_back(GatherItem{d.src, d.n, (int)gather_used});
+        scatter.push_back({d.host_dst, {gather_used, d.n}});
+        gather_used += d.n;
+      }
+      LAUNCH(ctx, kb_gather, n, 64, 0, upload(v), slot.gather.p);
+      break;
+    }
+    default: throw Error(DFTK_B200_EINVAL, "batched LOBPCG: unknown operation");
   }
-};
+}
+void BatchExec::issue(std::vector<Coro*>& coros) {
+  bool any = false;
+  for (auto& c : coros) any = any || c->cursor < c->ops.size();
+  if (!any) return;
+  rounds++;
+  std::vector<Op*> batch;
+  while (true) {
+    // count the operation types at the cursors; run the rarest one first so that solves that are an operation behind
+    // (a retry, a re-randomised column) catch up with the pack
+    int count[OP_NTYPES] = {0};
+    for (auto& c : coros)
+      if (c->cursor < c->ops.size()) count[c->ops[c->cursor].type]++;
+    int best = -1;
+    for (int t = 0; t < OP_NTYPES; ++t)
+      if (count[t] > 0 && (best < 0 || count[t] < count[best])) best = t;
+    if (best < 0) break;
+    batch.clear();
+    for (auto& c : coros)
+      if (c->cursor < c->ops.size() && c->ops[c->cursor].type == best) batch.push_back(&c->ops[c->cursor++]);
+    launch(best, batch);
+  }
+  if (gather_used)
+    CUDA_CHECK(cudaMemcpyAsync(slot.gather_h, slot.gather.p, gather_used * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_CHECK(cudaEventRecord(slot.ev, ctx->stream));
+  in_flight = true;
+}
+void BatchExec::complete(std::vector<Coro*>& coros) {
+  if (!in_flight) return;
+  CUDA_CHECK(cudaEventSynchronize(slot.ev));
+  in_flight = false;
+  for (auto& s : scatter) memcpy(s.first, slot.gather_h + s.second.first, s.second.second * sizeof(double));
+  scatter.clear();
+  gather_used = 0;
+  slot.ring.rewind();
+  for (auto& c : coros) {
+    c->ops.clear();
+    c->cursor = 0;
+  }
+}
 
 // ------------------------------------------------------------------ solver object
 struct SolveArgs {
@@ -1452,7 +1364,7 @@ static void run_batched(dftk_b200_ctx* ctx, std::vector<Lobpcg>& L, std::vector<
   std::vector<Coro*> members[2];
   for (int64_t i = 0; i < n_blocks; ++i) members[i % G].push_back(coros[i].get());   // interleaved: similar work per group
   std::unique_ptr<BatchExec> exec[2];
-  for (int g = 0; g < G; ++g) exec[g].reset(new BatchExec(ctx, g));
+  for (int g = 0; g < G; ++g) exec[g].reset(new BatchExec(ctx, ctx->slot[g]));
   auto stream_of = [&](int g) { return pipelined ? ctx->batch_streams[g] : user; };
   std::string first_err;
   int first_code = 0;
@@ -1608,15 +1520,13 @@ void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* co
                          double* ekin_host, double* enl_host) {
   if (n <= 0) return;
   dftk_b200_ctx* ctx = kbs[0]->grid->ctx;
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < (size_t)std::max<int64_t>(n, 256)) exec.reset_counters((size_t)n);
+  BatchExec exec(ctx, ctx->slot[0]);
   std::vector<KinDotsItem> kd;
   std::vector<GramItem> gr;
   std::vector<NlEnergyItem> ne;
   std::vector<GatherItem> ga;
   size_t used = 0;
   std::vector<std::pair<double*, std::pair<size_t, int>>> scatter;
-  int max_cols = 1;
   for (int64_t i = 0; i < n; ++i) {
     dftk_b200_kblock* kb = kbs[i];
     const int nb = n_bands[i];
@@ -1624,7 +1534,6 @@ void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* co
     if (nb == 0) continue;
     REQUIRE(nb <= SMALL_MAX_N && kb->n_proj <= SMALL_MAX_COLS, "band_energies_multi: block too large for the batched path");
     double* sc = kb->scal.ensure(2 * SMALL_MAX_N + 8);
-    max_cols = std::max(max_cols, nb);
     if (ekin_host) {
       REQUIRE(kb->has_kin, "band_energies: no kinetic term");
       kd.push_back(KinDotsItem{psi[i], (long long)kb->n_pw, (long long)kb->n_pw, nb, kb->kin.p, sc});
@@ -1645,18 +1554,20 @@ void band_energies_multi(int64_t n, dftk_b200_kblock* const* kbs, const cplx* co
       }
     }
   }
-  REQUIRE(used <= exec.gather_cap, "band_energies_multi: gather buffer too small");
-  if (!kd.empty()) LAUNCH(ctx, kb_kin_dots, dim3((unsigned)max_cols, (unsigned)kd.size()), 256, 0, exec.upload(kd));
+  REQUIRE(used <= BatchSlot::GATHER_CAP, "band_energies_multi: gather buffer too small");
+  BatchSlot& slot = ctx->slot[0];
+  if (!kd.empty()) exec.kin_dots_batch(kd);
   if (!gr.empty()) {
     exec.gram_batch(gr);
     LAUNCH(ctx, kb_nl_energy, (unsigned)ne.size(), 64, 0, exec.upload(ne));
   }
   if (!ga.empty()) {
-    LAUNCH(ctx, kb_gather, (unsigned)ga.size(), 64, 0, exec.upload(ga), ctx->batch_gather.p);
-    CUDA_CHECK(cudaMemcpyAsync(exec.gather_h, ctx->batch_gather.p, used * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    LAUNCH(ctx, kb_gather, (unsigned)ga.size(), 64, 0, exec.upload(ga), slot.gather.p);
+    CUDA_CHECK(cudaMemcpyAsync(slot.gather_h, slot.gather.p, used * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   }
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  for (auto& sct : scatter) memcpy(sct.first, exec.gather_h + sct.second.first, sct.second.second * sizeof(double));
+  slot.ring.rewind();
+  for (auto& sct : scatter) memcpy(sct.first, slot.gather_h + sct.second.first, sct.second.second * sizeof(double));
 }
 
 struct OrbOccItem { const cplx* a; int nb, spin; const double* w; };
@@ -1693,12 +1604,13 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
   dftk_b200_ctx* ctx = kbs[0]->grid->ctx;
   const int64_t n_orb = kbs[0]->n_orb;
   REQUIRE(n_orb > 0, "orbital_occupation_multi: the k-blocks have no orbitals (kblock_set_orbitals)");
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < (size_t)std::max<int64_t>(n, 256)) exec.reset_counters((size_t)n);
-  // the weights get a buffer of their own: the descriptor ring is recycled whenever it fills up
-  DevBuf<double>& wbuf = kbs[0]->wts;
-  wbuf.upload(occ_w_host, (size_t)n * ld_w, ctx->stream);
-  const double* w_dev = wbuf.p;
+  BatchExec exec(ctx, ctx->slot[0]);
+  // the weights are read by the last launch: the ring takes them and the descriptors of both launches without wrapping
+  DescRing& ring = ctx->slot[0].ring;
+  const size_t w_bytes = (size_t)n * ld_w * sizeof(double);
+  ring.reserve(DescRing::padded(w_bytes) + DescRing::padded(n * sizeof(GramItem)) + DescRing::padded(n * sizeof(OrbOccItem)),
+               ctx->stream);
+  const double* w_dev = (const double*)ring.put(occ_w_host, w_bytes, ctx->stream);
   std::vector<GramItem> gr;
   std::vector<OrbOccItem> items;
   int n_spin = 1;
@@ -1724,6 +1636,7 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
            (int)n_orb, n_spin, n_out);
   }
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ring.rewind();
 }
 
 // C (nA x nB, host, column-major) = A' B for tall column-major blocks (n_rows >> nA, nB <= SMALL_MAX_COLS): one fused launch
@@ -1732,73 +1645,13 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
 void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
                cplx* out_host) {
   REQUIRE(nA >= 1 && nB >= 1 && nA <= SMALL_MAX_COLS && nB <= SMALL_MAX_COLS, "tall_gram: 1 <= columns <= 96");
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < 256) exec.reset_counters(256);
-  cplx* C = (cplx*)ctx->batch_gather.p;       // >= 96 x 96 complex fit the gather buffer
+  BatchExec exec(ctx, ctx->slot[0]);
+  cplx* C = (cplx*)ctx->slot[0].gather.p;       // >= 96 x 96 complex fit the gather buffer
   std::vector<GramItem> v{single_gram_item(ctx, A, lda, nA, B, ldb, nB, n_rows, C)};
   exec.gram_batch(v);
   CUDA_CHECK(cudaMemcpyAsync(out_host, C, (size_t)nA * nB * sizeof(cplx), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-}
-
-// ------------------------------------------------------------------ direct minimisation (dm.cu)
-// The batched small-matrix kernels of the scheduler, for all blocks of <= SMALL_MAX_N bands in one launch each.  Every
-// call synchronises the stream before it returns: its descriptors are staged in the executor's pinned ring.
-void dm_small_gram(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* A, const cplx* const* B, int nb,
-                   cplx* C) {
-  REQUIRE(nb <= SMALL_MAX_N, "dm_small_gram: too many bands");
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < (size_t)std::max(n, 256)) exec.reset_counters((size_t)n);
-  std::vector<GramItem> v;
-  for (int i = 0; i < n; ++i) v.push_back(single_gram_item(ctx, A[i], kbs[i]->n_pw, nb, B[i], kbs[i]->n_pw, nb, kbs[i]->n_pw, C + (size_t)i * nb * nb));
-  exec.gram_batch(v);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-}
-
-void dm_small_times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* Y, const cplx* M, int nb,
-                    cplx* const* out, double alpha, double beta) {
-  REQUIRE(nb <= SMALL_MAX_N, "dm_small_times: too many bands");
-  BatchExec exec(ctx);
-  std::vector<BtimesItem> v;
-  for (int i = 0; i < n; ++i) v.push_back(single_btimes_item(Y[i], nb, M + (size_t)i * nb * nb, nb, out[i], kbs[i]->n_pw, alpha, beta));
-  exec.btimes_batch(v);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-}
-
-void dm_small_heev(dftk_b200_ctx* ctx, int n, cplx* G, int nb, double* w, cplx* V, double* stats) {
-  REQUIRE(nb <= SMALL_MAX_N, "dm_small_heev: too many bands");
-  BatchExec exec(ctx);
-  std::vector<Op> ops(n);
-  std::vector<Op*> p;
-  for (int i = 0; i < n; ++i) {
-    ops[i].type = OP_HEEV;
-    ops[i].u.heev = HeevItem{G + (size_t)i * nb * nb, nb, nb, w + (size_t)i * nb, V + (size_t)i * nb * nb, stats + 2 * i, nullptr, 0};
-    p.push_back(&ops[i]);
-  }
-  exec.launch(OP_HEEV, p);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-}
-
-void dm_kin_dots(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* X, int nb, double* out) {
-  BatchExec exec(ctx);
-  std::vector<KinDotsItem> v;
-  for (int i = 0; i < n; ++i) v.push_back(KinDotsItem{X[i], kbs[i]->n_pw, kbs[i]->n_pw, nb, kbs[i]->kin.p, out + (size_t)i * nb});
-  LAUNCH(ctx, kb_kin_dots, dim3((unsigned)nb, (unsigned)n), 256, 0, exec.upload(v));
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-}
-
-void dm_apply_h(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* in, cplx* const* out, int nb) {
-  BatchExec exec(ctx);
-  if (ctx->small_counter.cap < (size_t)std::max(n, 256)) exec.reset_counters((size_t)n);
-  std::vector<Op> ops(n);
-  std::vector<Op*> p;
-  for (int i = 0; i < n; ++i) {
-    ops[i].type = OP_APPLYH;
-    ops[i].u.applyh = ApplyHItem{kbs[i], in[i], out[i], nb};
-    p.push_back(&ops[i]);
-  }
-  exec.launch(OP_APPLYH, p);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ctx->slot[0].ring.rewind();
 }
 
 // One k-block solved by all ranks of the context together (single-k multi-GPU): X (n_pw x M, identical on every rank on

@@ -3,37 +3,11 @@
 // and host synchronisations instead of paying them one k-block at a time (reference seam: the independent per-k solves
 // of src/eigen/diag.jl:16-52).  The per-item work is the single-problem body: lobpcg_small.cuh for the small dense
 // algebra, item_body below for the elementwise and reduction operations, which the direct solver path launches for one
-// item through k_item.  Item descriptors live in a device-side ring that the host fills per launch.
+// item through k_item.  Item descriptors (batch_exec.cuh) live in a device-side ring that the host fills per launch.
 #pragma once
-#include "lobpcg_small.cuh"
+#include "batch_exec.cuh"
 
 namespace dftk {
-
-struct GramItem {
-  SmallMatList A, B;
-  long long rows_per_cta, n_rows;
-  int n_ctas, upper_only;
-  cplx* ws;            // n_ctas x (nA nB) partials of this item
-  cplx* C;
-  long long ldc;
-  unsigned* counter;   // arrival counter of this item (zero between launches)
-};
-struct CholItem { const cplx* O; long long ldo; int n; cplx* invR; long long ldi; double* stats; };
-struct RmulItem { cplx* X; long long ld, n_rows; int n; const cplx* invR; long long ldr; };
-struct BtimesItem { SmallMatList Y; const cplx* cm; long long ldcm; int ncols; cplx* out; long long ldo, n_rows; double alpha, beta; };
-struct HeevItem { cplx* G; long long ldg; int n; double* w; cplx* V; double* stats; double* lam_out; int n_keep; };
-struct ResidualItem { const cplx* AX; const cplx* X; const double* lam; cplx* R; long long ld, n_rows; int n_cols, squared; const double* kin; double* norms; double* meankin; };
-struct PrecondItem { cplx* R; long long ld, n_rows; int n_cols; const double* kin; const double* meankin; };
-struct ColnormItem { const cplx* X; long long ld, n_rows; int n_cols, squared; double* norms; };
-struct ScaleItem { cplx* X; long long ld, n_rows; int n_cols; const double* norms; };
-struct Copy2dItem { cplx* dst; long long ldd; const cplx* src; long long lds, n_rows; int n_cols; };   // src == nullptr: zero fill
-struct MakecpItem { cplx* cP; const cplx* cX; long long ld; int n_rows, n_cols, c0, lenXn; };
-struct StatsItem { const cplx* A; long long ld; int n_rows, n_cols; double* stats; };
-struct RandnItem { cplx* x; long long n_rows; unsigned long long seed; };
-struct LambdaItem { const cplx* X; const cplx* AX; long long ld, n_rows; int n_cols; double* lam; };
-struct GatherItem { const double* src; int n; int offset; };
-struct KinDotsItem { const cplx* X; long long ld, n_rows; int n_cols; const double* kin; double* out; };
-struct NlEnergyItem { const cplx* proj; const cplx* D; int np, nb; double* out; };
 
 extern __shared__ __align__(16) unsigned char batch_dyn_smem[];
 

@@ -38,15 +38,6 @@ unsigned ov_grid(dftk_b200_ctx* ctx, long long total) {
   return (unsigned)std::max<long long>(1, std::min<long long>(g, (long long)ctx->sm_count * 32));
 }
 
-void check_on_ctx(dftk_b200_ctx* ctx, const void* p, const char* what) {
-  cudaPointerAttributes a;
-  const cudaError_t e = cudaPointerGetAttributes(&a, p);
-  if (e != cudaSuccess) cudaGetLastError();
-  REQUIRE(p && e == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged),
-          std::string(what) + ": arrays must be device memory");
-  REQUIRE(a.device == ctx->device, std::string(what) + ": arrays must be on the context's device");
-}
-
 // one pair at a time: gather B_p[idx_p] (n_b x n_G) into scratch, then C_p = A_p^H gathered on the DMMA ZGEMM
 void overlap_large(dftk_b200_ctx* ctx, int64_t n_pairs, int64_t n_a, int64_t n_b, const void* const* A, const int64_t* ld_a,
                    const int64_t* n_G, const void* const* B, const int64_t* ld_b, const int64_t* const* idx, cplx* Cd,
@@ -84,14 +75,14 @@ int dftk_b200_overlap_multi(dftk_b200_ctx* ctx, int64_t n_pairs, int64_t n_a, in
   if (n_pairs == 0) return DFTK_B200_OK;
   REQUIRE(A && ld_a && n_G && B && ld_b, "overlap_multi: NULL argument list");
   REQUIRE((long long)n_a * n_b <= (1LL << 30), "overlap_multi: blocks too large");
-  check_on_ctx(ctx, C, "overlap_multi");
+  require_device(ctx, C, "overlap_multi: arrays");
   long long max_nG = 0;
   for (int64_t p = 0; p < n_pairs; ++p) {
     const bool ident = !idx || !idx[p];
     REQUIRE(n_G[p] >= 0 && ld_a[p] >= n_G[p] && ld_b[p] >= 1 && (!ident || ld_b[p] >= n_G[p]), "overlap_multi: bad sizes");
-    check_on_ctx(ctx, A[p], "overlap_multi");
-    check_on_ctx(ctx, B[p], "overlap_multi");
-    if (!ident && n_G[p] > 0) check_on_ctx(ctx, idx[p], "overlap_multi");
+    require_device(ctx, A[p], "overlap_multi: arrays");
+    require_device(ctx, B[p], "overlap_multi: arrays");
+    if (!ident && n_G[p] > 0) require_device(ctx, idx[p], "overlap_multi: arrays");
     max_nG = std::max<long long>(max_nG, n_G[p]);
   }
   const long long nab = n_a * n_b;
@@ -114,17 +105,18 @@ int dftk_b200_overlap_multi(dftk_b200_ctx* ctx, int64_t n_pairs, int64_t n_a, in
   const long long want = (8LL * ctx->sm_count + n_groups - 1) / n_groups;
   const int n_chunks = (int)std::max<long long>(1, std::min<long long>({want, (max_nG + OV_ROWS - 1) / OV_ROWS, OV_MAX_CHUNKS}));
   REQUIRE(n_groups <= 0x7fffffffLL, "overlap_multi: too many pairs");
-  const size_t gbytes = groups.size() * sizeof(OvGroup), pbytes = pairs.size() * sizeof(OvPair);
-  char* d = ctx->ov_items.ensure(gbytes + pbytes);
-  CUDA_CHECK(cudaMemcpyAsync(d, groups.data(), gbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CUDA_CHECK(cudaMemcpyAsync(d + gbytes, pairs.data(), pbytes, cudaMemcpyHostToDevice, ctx->stream));
+  DescRing& ring = ctx->slot[0].ring;
+  ring.reserve(DescRing::padded(groups) + DescRing::padded(pairs), ctx->stream);
+  const OvGroup* d_groups = ring.put(groups, ctx->stream);
+  const OvPair* d_pairs = ring.put(pairs, ctx->stream);
   cplx* ws = ctx->ov_ws.ensure((size_t)n_chunks * n_pairs * nab);
   const size_t smem = (size_t)ov_smem_entries((int)n_a, (int)n_b) * sizeof(cplx);
   CUDA_CHECK(cudaFuncSetAttribute(k_ov_partial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LAUNCH(ctx, k_ov_partial, dim3((unsigned)n_groups, (unsigned)n_chunks), OV_THREADS, smem, (const OvGroup*)d,
-         (const OvPair*)(d + gbytes), n_chunks, (int)n_a, (int)n_b, (long long)n_pairs, ws);
+  LAUNCH(ctx, k_ov_partial, dim3((unsigned)n_groups, (unsigned)n_chunks), OV_THREADS, smem, d_groups, d_pairs, n_chunks, (int)n_a,
+         (int)n_b, (long long)n_pairs, ws);
   LAUNCH(ctx, k_ov_reduce, ov_grid(ctx, n_pairs * nab), OV_THREADS, 0, (const cplx*)ws, n_chunks, (long long)n_pairs, (int)nab, Cd);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));   // the descriptor vectors are released on return
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ring.rewind();
   API_END(ctx)
 }
 

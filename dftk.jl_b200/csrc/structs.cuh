@@ -106,7 +106,6 @@ struct dftk_b200_kblock {
   dftk::DevBuf<dftk::cplx> lobpcg_ws; // big LOBPCG workspace
   dftk::DevBuf<dftk::cplx> small_ws;  // small dense LOBPCG workspace
   dftk::DevBuf<dftk::cplx> slab_x, slab_stage;   // slab-distributed solve (lobpcg_run_slab): this rank's rows of X, reassembly staging
-  dftk::DevBuf<double> wts;
   dftk::DevBuf<double> scal;          // per-block scalars of a LOBPCG solve (several blocks are solved side by side)
 };
 
@@ -123,7 +122,7 @@ void kb_apply_local_kinetic(dftk_b200_kblock* kb, const cplx* psi, cplx* hpsi, i
 // the same for several k-blocks of ONE grid in five launches in total; returns false (nothing done) when the blocks do
 // not qualify (different grids, generic FFT engine, missing potential / kinetic term): the caller then loops
 bool kb_apply_local_kinetic_multi(int n, dftk_b200_kblock* const* kbs, const cplx* const* psi, cplx* const* hpsi,
-                                  const int* n_bands, const void* (*upload)(void* self, const void* host, size_t bytes), void* self);
+                                  const int* n_bands, DescRing& ring);
 void kb_sphere_to_real(dftk_b200_kblock* kb, const cplx* psi, cplx* cube, int64_t n_bands, double scale);
 void kb_real_to_sphere(dftk_b200_kblock* kb, const cplx* cube, cplx* out, int64_t n_bands, double scale);
 void kb_density_accumulate(dftk_b200_kblock* kb, const cplx* psi, const double* occ_w_host,
@@ -208,13 +207,4 @@ void orbital_occupation_multi(int64_t n, dftk_b200_kblock* const* kbs, const cpl
 void tall_gram(dftk_b200_ctx* ctx, const cplx* A, int64_t lda, int nA, const cplx* B, int64_t ldb, int nB, int64_t n_rows,
                cplx* out_host);
 void lobpcg_set_attributes();
-// direct minimisation (dm.cu): the scheduler's batched small-matrix kernels on blocks of <= SMALL_MAX_N bands, all blocks at
-// once (C_i, M_i, G_i: nb x nb at offset i nb^2); dm_kin_dots and dm_apply_h take any band count
-void dm_small_gram(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* A, const cplx* const* B, int nb,
-                   cplx* C);                                                       // C_i = A_i^H B_i
-void dm_small_times(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* Y, const cplx* M, int nb,
-                    cplx* const* out, double alpha, double beta);                  // out_i = alpha Y_i M_i + beta out_i
-void dm_small_heev(dftk_b200_ctx* ctx, int n, cplx* G, int nb, double* w, cplx* V, double* stats);   // eigenvectors -> G_i
-void dm_kin_dots(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* X, int nb, double* out);
-void dm_apply_h(dftk_b200_ctx* ctx, int n, dftk_b200_kblock* const* kbs, const cplx* const* in, cplx* const* out, int nb);
 }  // namespace dftk

@@ -78,10 +78,6 @@ void check_cube(int nx, int ny, int nz, const char* what) {
   REQUIRE(nx >= 1 && ny >= 1 && nz >= 1, std::string(what) + ": cube sizes must be positive");
 }
 
-void check_dev_ptr(const void* p, const char* what) {
-  REQUIRE(p && is_device_ptr(p), std::string(what) + ": arrays must be device memory");
-}
-
 }  // namespace
 
 extern "C" {
@@ -93,10 +89,10 @@ int dftk_b200_remap_tables(dftk_b200_ctx* ctx, int64_t n_G, const int64_t* G, co
   check_cube(nx, ny, nz, "remap_tables");
   REQUIRE(!is_device_ptr(M) && !is_device_ptr(delta) && !(tau && is_device_ptr(tau)), "remap_tables: M, delta and tau are host arrays");
   if (n_G == 0) return DFTK_B200_OK;
-  check_dev_ptr(G, "remap_tables");
-  check_dev_ptr(lookup, "remap_tables");
-  check_dev_ptr(idx, "remap_tables");
-  if (phase) check_dev_ptr(phase, "remap_tables");
+  require_device(ctx, G, "remap_tables: arrays");
+  require_device(ctx, lookup, "remap_tables: arrays");
+  require_device(ctx, idx, "remap_tables: arrays");
+  if (phase) require_device(ctx, phase, "remap_tables: arrays");
   TrTableArgs a;
   for (int i = 0; i < 9; ++i) a.M[i] = M[i];
   for (int i = 0; i < 3; ++i) {
@@ -122,10 +118,10 @@ int dftk_b200_sphere_remap(dftk_b200_ctx* ctx, int64_t n_pairs, const void* cons
     REQUIRE(n_bands[p] >= 0 && n_dst[p] >= 0 && ld_dst[p] >= n_dst[p] && ld_src[p] >= 0 && (!row_offset || row_offset[p] >= 0),
             "sphere_remap: bad sizes");
     if (n_bands[p] == 0 || n_dst[p] == 0) continue;
-    check_dev_ptr(src[p], "sphere_remap");
-    check_dev_ptr(dst[p], "sphere_remap");
-    check_dev_ptr(idx[p], "sphere_remap");
-    if (phase && phase[p]) check_dev_ptr(phase[p], "sphere_remap");
+    require_device(ctx, src[p], "sphere_remap: arrays");
+    require_device(ctx, dst[p], "sphere_remap: arrays");
+    require_device(ctx, idx[p], "sphere_remap: arrays");
+    if (phase && phase[p]) require_device(ctx, phase[p], "sphere_remap: arrays");
     items.push_back(TrRemapItem{(const cplx*)src[p], (cplx*)dst[p], (const long long*)idx[p],
                                 phase ? (const cplx*)phase[p] : nullptr, (long long)ld_src[p], (long long)ld_dst[p],
                                 row_offset ? (long long)row_offset[p] : 0, (long long)n_dst[p], (long long)n_bands[p]});
@@ -133,14 +129,13 @@ int dftk_b200_sphere_remap(dftk_b200_ctx* ctx, int64_t n_pairs, const void* cons
     max_bands = std::max<long long>(max_bands, n_bands[p]);
   }
   if (items.empty()) return DFTK_B200_OK;
-  const size_t bytes = items.size() * sizeof(TrRemapItem);
-  char* d = ctx->tr_items.ensure(bytes);
-  CUDA_CHECK(cudaMemcpyAsync(d, items.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+  const TrRemapItem* d = ctx->slot[0].ring.put(items, ctx->stream);
   const unsigned gx = (unsigned)std::min<long long>((max_dst + TR_THREADS - 1) / TR_THREADS, 65535);
   const unsigned gz = (unsigned)((max_bands + TR_BAND_GROUP - 1) / TR_BAND_GROUP);
   REQUIRE(gz <= 65535, "sphere_remap: too many bands");
-  LAUNCH(ctx, k_sphere_remap, dim3(gx, (unsigned)items.size(), gz), TR_THREADS, 0, (const TrRemapItem*)d);
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));   // the descriptor vector is released on return
+  LAUNCH(ctx, k_sphere_remap, dim3(gx, (unsigned)items.size(), gz), TR_THREADS, 0, d);
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  ctx->slot[0].ring.rewind();
   API_END(ctx)
 }
 
@@ -151,8 +146,8 @@ int dftk_b200_fourier_block_copy(dftk_b200_ctx* ctx, const void* in, int nx_in, 
   check_cube(nx_in, ny_in, nz_in, "fourier_block_copy");
   check_cube(nx_out, ny_out, nz_out, "fourier_block_copy");
   if (batch == 0) return DFTK_B200_OK;
-  check_dev_ptr(in, "fourier_block_copy");
-  check_dev_ptr(out, "fourier_block_copy");
+  require_device(ctx, in, "fourier_block_copy: arrays");
+  require_device(ctx, out, "fourier_block_copy: arrays");
   REQUIRE(in != out, "fourier_block_copy: in and out must not alias");
   const long long No = (long long)nx_out * ny_out * nz_out;
   LAUNCH(ctx, k_block_copy, dim3(tr_grid(ctx, No), (unsigned)batch), TR_THREADS, 0, (const cplx*)in, nx_in, ny_in, nz_in,
@@ -165,7 +160,7 @@ int dftk_b200_bspline2_prefilter(dftk_b200_ctx* ctx, void* f, int nx, int ny, in
   REQUIRE(ctx && batch >= 0, "bspline2_prefilter: bad argument");
   check_cube(nx, ny, nz, "bspline2_prefilter");
   if (batch == 0) return DFTK_B200_OK;
-  check_dev_ptr(f, "bspline2_prefilter");
+  require_device(ctx, f, "bspline2_prefilter: arrays");
   LAUNCH(ctx, k_bspline_prefilter, tr_grid(ctx, (long long)nx * ny * nz), TR_THREADS, 0, (cplx*)f, nx, ny, nz, (long long)batch);
   API_END(ctx)
 }
@@ -181,8 +176,8 @@ int dftk_b200_bspline2_evaluate(dftk_b200_ctx* ctx, const double* f, int nx, int
     REQUIRE((long long)nx * rep[0] == nx_out && (long long)ny * rep[1] == ny_out && (long long)nz * rep[2] == nz_out,
             "bspline2_evaluate: direct sampling needs n_out = rep * n_in on every axis");
   if (batch == 0) return DFTK_B200_OK;
-  check_dev_ptr(f, "bspline2_evaluate");
-  check_dev_ptr(out, "bspline2_evaluate");
+  require_device(ctx, f, "bspline2_evaluate: arrays");
+  require_device(ctx, out, "bspline2_evaluate: arrays");
   REQUIRE((const void*)f != (const void*)out, "bspline2_evaluate: in and out must not alias");
   TrRep r{{rep[0], rep[1], rep[2]}};
   const long long No = (long long)nx_out * ny_out * nz_out;
